@@ -7,7 +7,7 @@ One "step" = one full gradient evaluation of the ensemble: forward solve + fused
 reduction (+ the one all-reduce of dp over ranks for N>1, issued by b200adj_reverse itself through the handle's NCCL
 communicator; members are sharded, weak scaling: 65536 per GPU).
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--members M]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--members M] [--dump-outputs DIR]
   python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P bench.py --gpus N ...
 
 Keys of the one JSON line (rank 0):
@@ -58,8 +58,8 @@ def c2_config(world, members_per_gpu, block):
     return {"workload": "C2 Lorenz d=3 P=3 N=65536/GPU GaussAdjoint Tsit5 fixed dt=0.01 T=10 saveat=0.1 dgdu=u-2 shared p",
             "members_per_gpu": members_per_gpu, "S": int(round(W["T"] / W["dt"])), "K": W["nsave"],
             "parallelism": f"ensemble-shard x{world}",
-            "l2": "per-step working set = 1.57 GB of checkpoints per GPU (>> 126 MB L2), no explicit flush",
-            "block_threads": block or "auto: ceil32(N / (n_SM * waves)) = 448, one block per SM"}
+            "l2": "per-step working set = 1.57 GB of checkpoints per GPU (>> 50 MB L2), no explicit flush",
+            "block_threads": block or "auto: ceil32(N / (n_SM * waves)) = 512 on 132 SMs, one block per SM"}
 
 
 def host_cores():
@@ -99,41 +99,30 @@ def best_threads():
     return _BEST_THREADS
 
 
-def profile_metric(fname, *names):
-    """metrics of a committed ncu summary (profiles/*.json, written by profiles/summarize.py); None when absent"""
-    try:
-        with open(os.path.join(ROOT, "profiles", fname)) as f:
-            m = json.load(f)
-        scale = {"Gbyte": 1e9, "Mbyte": 1e6, "Kbyte": 1e3, "byte": 1.0, "%": 1.0}
-        out = []
-        for n in names:
-            v = m[n]
-            out.append(v["value"] * scale.get(v.get("unit", ""), 1.0))
-        return out
-    except Exception:
-        return None
-
-
-def ncu_traffic():
-    """dram__bytes_read.sum + dram__bytes_write.sum of the reverse kernel per launch, from the committed ncu capture"""
-    for f in ("r2_reverse_ncu_summary.json", "r1_reverse_ncu_summary.json"):
-        v = profile_metric(f, "dram__bytes_read.sum", "dram__bytes_write.sum")
-        if v is not None:
-            return v[0] + v[1], f"profiles/{f} (ncu --set full of this command; not re-measured in this run)"
-    return None, None
-
-
 def peaks():
     path = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(path):
         with open(path) as f:
             m = json.load(f)
-        return m.get("hbm_gbs", 6650.0), m.get("bf16_tflops_sustained", 1426.0), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, 1426.0, "fallback (B200_PROFILING.md)"
+        return m.get("hbm_gbs", 3350.0), m.get("bf16_tflops_sustained", 989.0), "measured (MEASURED_PEAKS.json)"
+    return 3350.0, 989.0, "NVIDIA H100 SXM data sheet (HBM3 3.35 TB/s, dense BF16 989 TFLOP/s at 700 W), not measured"
+
+
+def gpu_identity(device):
+    """name and power limit of the card the numbers were measured on (a power-capped card clocks lower)"""
+    import torch
+    out = {"name": torch.cuda.get_device_name(device), "power_limit_w": None}
+    try:
+        res = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader,nounits", "-i", str(device)],
+                             capture_output=True, text=True, timeout=30)
+        out["power_limit_w"] = float(res.stdout.strip().splitlines()[0])
+    except Exception:
+        pass
+    return out
 
 
 class ClockSampler:
-    """nvidia-smi clocks/throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks/throttle reasons DURING the timed region."""
     Q = ("timestamp,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -522,6 +511,11 @@ def run_ours(args):
     ms_per_step = total_ms / args.steps
     value = N * world / (ms_per_step * 1e-3)
     dp_check = main.dp.cpu().numpy().tolist()
+    if args.dump_outputs and rank == 0:
+        # what the timed path computed in its last step: the gradient a caller of forward + reverse receives
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "du0.npy"), main.du0.cpu().numpy().astype(np.float64))
+        np.save(os.path.join(args.dump_outputs, "dp.npy"), main.dp.cpu().numpy().astype(np.float64))
     main.close()
 
     # ---------------- end-to-end arms: public API, host buffers ----------------
@@ -549,7 +543,7 @@ def run_ours(args):
             dist.all_reduce(te, op=dist.ReduceOp.MAX)
         return float(te.cpu()[0]), out
 
-    e2e_steps = max(1, min(args.steps, 10))
+    e2e_steps = args.steps
     e2e_s, (du0_e, dp_e) = time_host(step_e2e, e2e_steps, max(1, min(args.warmup, 3)))
     e2e_value = N * world / e2e_s
     h2d = u0_h.nbytes + p_h.nbytes
@@ -567,7 +561,7 @@ def run_ours(args):
         return pullback(delta_pin.numpy())
 
     step_rrule(fill=True)
-    rr_steps = max(1, min(args.steps, 5))
+    rr_steps = args.steps
     rr_s, tang = time_host(step_rrule, rr_steps, 1)
     rr_ok = bool(np.allclose(np.asarray(tang[4]).ravel(), np.asarray(dp_check), rtol=1e-10))
     kd = W["nsave"] * 3 * N * 8
@@ -590,11 +584,11 @@ def run_ours(args):
     # ---------------- secondary BASELINE configs, sharded over the same ranks ----------------
     secondary = {}
     if not args.no_secondary and not args.members:
-        sec_steps, sec_warm = max(5, min(args.steps, 20)), 3
-        few = max(3, min(sec_steps, 5))
-        legs = [("c4", spec_c4, 4096, sec_steps, sec_warm, True), ("c4_full", spec_c4, 18944 * world, sec_steps, sec_warm, False),
-                ("c5", spec_c5, 131072, sec_steps, sec_warm, True), ("c1_ensemble", spec_c1, 65536 * world, few, 2, True),
-                ("c3", spec_c3, 16384, few, 2, True)]
+        sec_steps, sec_warm = args.steps, 3
+        # c4_full: one 128-member CTA per SM of an H100 SXM (132 SMs)
+        legs = [("c4", spec_c4, 4096, sec_steps, sec_warm, True), ("c4_full", spec_c4, 16896 * world, sec_steps, sec_warm, False),
+                ("c5", spec_c5, 131072, sec_steps, sec_warm, True), ("c1_ensemble", spec_c1, 65536 * world, sec_steps, 2, True),
+                ("c3", spec_c3, 16384, sec_steps, 2, True)]
         for key, mk, n_total, k_steps, k_warm, with_par in legs:
             try:
                 secondary[key] = secondary_leg(mk(), n_total, rank, world, local, k_steps, k_warm, barrier, threads, with_parity=with_par)
@@ -612,12 +606,9 @@ def run_ours(args):
         I = DP_INSTR_PER_MEMBER_STEP
         flops = (2 * I["dfma"] + I["dmul"] + I["dadd"]) * float(N) * S
         dp_issue = (I["dfma"] + I["dmul"] + I["dadd"]) * float(N) * S            # thread-level fp64 instructions per launch
-        sm_mhz = (clocks or {}).get("sm_mhz") or 1965.0
+        sm_mhz = (clocks or {}).get("sm_mhz") or 1980.0
         nsm = torch.cuda.get_device_properties(local).multi_processor_count
         fp64_peak_tf = nsm * 64 * 2 * sm_mhz * 1e6 / 1e12                         # 64 DFMA/clk/SM
-        pipe = profile_metric("r2_reverse_ncu_summary.json", "sm__inst_executed_pipe_fp64.avg.pct_of_peak_sustained_active") or \
-            profile_metric("r1_reverse_ncu_summary.json", "sm__inst_executed_pipe_fp64.avg.pct_of_peak_sustained_active")
-        traffic, traffic_src = ncu_traffic() if N == W["members_per_gpu"] else (None, None)
         cpu_sample = W["members_per_gpu"]
         cpu_oracle_rate(256, threads)                      # warm the library / thread pool
         cpu_rate, cpu_s = cpu_oracle_rate(cpu_sample, threads)
@@ -632,15 +623,14 @@ def run_ours(args):
                                                   "ncclAllReduce after the reverse kernel (the GPUs do not map each other)"),
             "roofline": {"bound": "hbm", "kernel": "tsit5_reverse_kernel<Lorenz,GAUSS>", "achieved": achieved, "peak": hbm,
                          "unit": "GB/s", "frac": achieved / hbm,
-                         "traffic": traffic, "traffic_source": traffic_src, "peak_source": peak_src,
+                         "peak_source": peak_src,
                          "algorithmic_bytes_per_launch": alg_bytes, "bytes_per_member_step": ALG_BYTES_PER_MEMBER_STEP,
                          "compulsory_bytes_per_launch": compulsory,
                          "compulsory_frac": compulsory / (rev_ms * 1e-3) / 1e9 / hbm,
                          "fp64": {"tflops": flops / (rev_ms * 1e-3) / 1e12, "peak_tflops": fp64_peak_tf,
                                   "frac": dp_issue / (rev_ms * 1e-3) / (nsm * 64 * sm_mhz * 1e6),
-                                  "pipe_active_pct_ncu": None if pipe is None else pipe[0],
                                   "note": "fp64 pipe: 64 DFMA/clk/SM at the SM clock sampled in this run; frac = issued DFMA+DMUL+DADD / pipe slots "
-                                          "(426 per member-step, counted in SASS); pipe_active from the committed ncu capture"},
+                                          "(426 per member-step, counted in SASS)"},
                          "note": "per-step accounting of SURVEY 8d (state counted as if it lived in HBM between steps); the time "
                                  "loop is in-kernel so real DRAM traffic is the compulsory stream (compulsory_frac of the HBM peak); "
                                  "the binding resource is the fp64 FMA pipe (fp64.frac)"},
@@ -654,6 +644,7 @@ def run_ours(args):
                           "api": "_concrete_solve_adjoint(prob, Tsit5, B200Adjoint(GaussAdjoint)) -> host primal sol.u[K,d,N]; pullback(host Delta[K,d,N])",
                           "matches_device_arm": rr_ok},
             "gpu_launches": int(launches),
+            "gpu": gpu_identity(local),
             "clocks": clocks,
             "dp": dp_check,
             "parity": parity,
@@ -821,6 +812,8 @@ def main():
     ap.add_argument("--dtype", default="", help="c4 only: bf16_f32acc (default), f32 or f64")
     ap.add_argument("--no-secondary", action="store_true", help="skip the sharded C4 / C5 legs (profiling runs)")
     ap.add_argument("--nccl-allreduce", action="store_true", help="N > 1: ncclAllReduce instead of the fused peer-memory all-reduce (A/B)")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="write du0.npy and dp.npy (float64) of the last timed step of the headline workload to DIR")
     args = ap.parse_args()
     if args.warmup < 3 and args.impl == "ours":
         args.warmup = 3

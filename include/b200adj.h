@@ -1,5 +1,5 @@
 /*
- * b200adj.h -- C ABI of libb200adj.so, the B200-native (sm_100a) ensemble continuous-adjoint engine.
+ * b200adj.h -- C ABI of libb200adj.so, the Hopper-native (H100, sm_90a) ensemble continuous-adjoint engine.
  *
  * This is the drop-in boundary for ONE hot path of SciML/SciMLSensitivity.jl v7.112.3: the reverse-mode
  * continuous adjoint (InterpolatingAdjoint / GaussAdjoint / QuadratureAdjoint / BacksolveAdjoint) evaluated

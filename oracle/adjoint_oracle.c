@@ -3,7 +3,7 @@
  *
  * CPU restatement (plain C, fp64, OpenMP over ensemble members) of the reverse-mode
  * continuous-adjoint hot path of SciML/SciMLSensitivity.jl v7.112.3.  It is the CHECKER
- * for the B200 kernels: only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline /
+ * for the device kernels: only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline /
  * --impl reference legs may load it.  The product path (libb200adj.so) never links or calls it.
  *
  * PARITY STATUS: pinned by the literal results the reference itself holds for this path, "parity unpinned"

@@ -1,7 +1,7 @@
-"""scimlsensitivity.jl_b200 -- B200-native ensemble continuous-adjoint engine.
+"""scimlsensitivity.jl_b200 -- H100-native (Hopper) ensemble continuous-adjoint engine.
 
 One hot path of SciML/SciMLSensitivity.jl (reverse-mode continuous adjoints over an EnsembleProblem) rebuilt as
-hand-written sm_100a CUDA kernels behind a C ABI (include/b200adj.h), with this thin host layer mirroring the
+hand-written sm_90a CUDA kernels behind a C ABI (include/b200adj.h), with this thin host layer mirroring the
 reference's `sensealg=` plugin surface.  Import as `scimlsensitivity_jl_b200` (the directory name carries a dot).
 """
 from . import _lib

@@ -55,7 +55,7 @@ def nvcc_path():
 
 
 def build(force=False, verbose=False):
-    """Compile csrc/*.cu for sm_100a into scimlsensitivity.jl_b200/libb200adj.so (in-tree, travels with gpurun)."""
+    """Compile csrc/*.cu for sm_90a into scimlsensitivity.jl_b200/libb200adj.so (in-tree, next to the package)."""
     from concurrent.futures import ThreadPoolExecutor
     srcs = [os.path.join(_CSRC, f) for f in sorted(os.listdir(_CSRC)) if f.endswith((".cu", ".cuh", ".inc", ".h"))]
     srcs.append(os.path.join(_ROOT, "include", "b200adj.h"))
@@ -64,7 +64,7 @@ def build(force=False, verbose=False):
     cus = [s for s in srcs if s.endswith(".cu")]
     objdir = os.path.join(_PKG, "build")
     os.makedirs(objdir, exist_ok=True)
-    flags = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC", "-Xptxas", "-v"]
+    flags = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC", "-Xptxas", "-v"]
 
     def deps(cu):
         """headers a translation unit includes, transitively (quoted includes inside csrc/ and include/)"""

@@ -1,4 +1,4 @@
-// api.cu -- C ABI (include/b200adj.h) of the B200-native ensemble continuous-adjoint engine.
+// api.cu -- C ABI (include/b200adj.h) of the H100-native (sm_90a) ensemble continuous-adjoint engine.
 // Handle management, validation, host<->device staging; kernel dispatch goes through handle.h into disp_*.cu.
 // No torch types, no CPU fallback.
 #include <dlfcn.h>
@@ -360,7 +360,7 @@ int32_t b200adj_create(const b200adj_cfg* cfg, void** handle) {
     // every few steps keep all warps of an SM in lockstep -- independent small blocks drift apart by >2x under the
     // highest-warp-id-first arbiter and the stragglers run the tail latency-bound), sized so that the blocks cover
     // the SMs evenly: block = ceil32(N / (nSM * waves)).
-    int nsm = 148;
+    int nsm = 132;
     cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, cfg->device);
     int block = cfg->block_threads;
     if (block == 0) {
@@ -414,7 +414,7 @@ int32_t b200adj_create(const b200adj_cfg* cfg, void** handle) {
     CREATE_TRY(cudaMalloc(&h->d_fwd_save_of_step, ((size_t)S + 1) * sizeof(int32_t)));
     CREATE_TRY(cudaMemcpy(h->d_fwd_save_of_step, sos.data(), ((size_t)S + 1) * sizeof(int32_t), cudaMemcpyHostToDevice));
     if (sde) CREATE_TRY(cudaMalloc(&h->d_noise, (size_t)S * m * N * e));
-    // BF16_F32ACC = mlp_tc.cuh: member and gradient GEMMs in the time loop on tcgen05, accumulators in TMEM
+    // BF16_F32ACC = mlp_tc.cuh: member and gradient GEMMs in the time loop on wgmma, fp32 accumulators in registers
     h->mlp_tc = mlp && cfg->dtype == B200ADJ_BF16_F32ACC;
     if (h->mlp_tc) CREATE_TRY(cudaMalloc(&h->d_kst, (size_t)S * 14 * N * sizeof(float)));
     if (cfg->flags & B200ADJ_FLAG_TRACE) {

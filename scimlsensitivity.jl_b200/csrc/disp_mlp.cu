@@ -1,4 +1,4 @@
-// disp_mlp.cu -- launchers of the MLP-family kernels: CUDA-core fp64 / fp32 (mlp.cuh) and the tcgen05 bf16 path (mlp_tc.cuh)
+// disp_mlp.cu -- launchers of the MLP-family kernels: CUDA-core fp64 / fp32 (mlp.cuh) and the wgmma bf16 path (mlp_tc.cuh)
 #include "handle.h"
 namespace b200adj {
 namespace {

@@ -30,7 +30,7 @@ struct Handle {
     std::vector<int32_t> save_of_step;
     int S = 0;
     int64_t Npad = 0;
-    int block = 64, grid = 0, nsm = 148;
+    int block = 64, grid = 0, nsm = 132;
     int ckpt_every = 1;               // fixed-step Tsit5: forward states kept every C steps, segments re-solved in the reverse pass
     cudaStream_t stream = nullptr, own_stream = nullptr;
     // device memory owned by the handle
@@ -55,7 +55,7 @@ struct Handle {
     bool has_dgdp = false, has_cdgdp = false;
     double dgdp_c[8] = {0}, dgdp_e[8] = {0}, cdgdp_c[8] = {0}, cdgdp_e[8] = {0};
     float* d_kst = nullptr;           // tensor-core MLP path: the forward stages of every step ([S][7][2][N] floats)
-    bool mlp_tc = false;              // BF16_F32ACC: every GEMM-shaped piece of the time loop on tcgen05 (mlp_tc.cuh)
+    bool mlp_tc = false;              // BF16_F32ACC: every GEMM-shaped piece of the time loop on wgmma (mlp_tc.cuh)
     double *r_ft = nullptr, *r_fu = nullptr, *r_fk = nullptr, *d_saveat = nullptr;
     // QuadratureAdjoint on the adaptive steppers (allocated at the first Quadrature reverse pass): member-major reverse dense
     // solution + member-major copy of the forward one (quadgk.cuh)

@@ -1,74 +1,143 @@
 // mlp_tc.cuh -- the neural-ODE family (BASELINE config C4, dtype BF16_F32ACC) with EVERY GEMM-shaped piece of the time loop on
-// the 5th-generation tensor cores: bf16 operands in shared memory, fp32 accumulators in TMEM, tcgen05.mma issued by one
-// thread, no operand tapes and no reduction over members on the CUDA cores.
+// the Hopper tensor cores: bf16 operands in shared memory, fp32 accumulators in the registers of the CTA's one warpgroup,
+// wgmma.mma_async issued by all 128 threads, no operand tapes and no reduction over members on the CUDA cores.
 //
-// Round-2 layout (the round-1 kernel put 128 members on one CTA, one thread per member: at the BASELINE size N = 4096 that is
-// 32 CTAs on 148 SMs, each a serial chain of 128 x 128 MUFU.TANH + MMA round trips per stage):
+// Narrow layout (at the BASELINE size N = 4096, one member per thread would be 32 CTAs on 132 SMs, each a serial chain of
+// 128 x 128 MUFU.TANH + MMA round trips per stage):
 //   one CTA = 32 ensemble members x 4 warps.  Thread (w, m) = warp w, lane m owns member m's feature QUARTER [16 w, 16 w + 16):
-//   16 tanh per layer instead of 64, 128 CTAs at N = 4096, two CTAs per SM at large N.  The M = 128 rows of every member MMA
-//   hold FOUR COPIES of the 32 member rows (row 32 c + m = member m), because a warp can only read the 32 TMEM lanes it owns:
-//   warp w reads its accumulator quarter from copy w (lane 32 w + m, columns 16 w ..).  The member state (u, lam, RK stages,
-//   d = 2) is kept redundantly by the 4 threads of a member; the two 2-vectors a stage returns (f, J'lam) are summed over the
+//   16 tanh per layer instead of 64, 128 CTAs at N = 4096, several CTAs per SM at large N.  The member MMAs have M = 64 rows:
+//   rows 0..31 are the members, rows 32..63 stay zero.  The accumulator fragment of rows 0..31 (warps 0 and 1) goes through a
+//   shared fp32 tile, from which thread (w, m) reads member m's columns 16 w ..  The member state (u, lam, RK stages, d = 2)
+//   is kept redundantly by the 4 threads of a member; the two 2-vectors a stage returns (f, J'lam) are summed over the
 //   quarters through shared memory.
 //
-//   member GEMMs (M = 128 = 4 x 32 members, N = 64, K = 64; K-major operands):
-//     forward   Z2 = H1 W2'          A = tile TB (H1, 4 copies),      B = W2   (n = out, k = in)
-//     backward  dH1 = dZ2 W2         A = tile TA (wt dZ2, 4 copies),  B = W2^T (n = in,  k = out)
-//   gradient GEMMs (K = the 32 members of copy 0; the SAME tiles read as MN-major operands -- element (m, f) of a member tile
-//   sits at (m/8) ROW + (f/8) 128 + (m%8) 16 + (f%8) 2, which is at once the canonical K-major layout of [member x feature] and
-//   the canonical MN-major layout of [feature x member]; probed by tuning/tc_probe.cu), accumulated in TMEM over the whole
-//   reverse pass:
+//   member GEMMs (M = 64, N = 64, K = 64; K-major operands):
+//     forward   Z2 = H1 W2'          A = tile TB (H1),      B = W2   (n = out, k = in)
+//     backward  dH1 = dZ2 W2         A = tile TA (wt dZ2),  B = W2^T (n = in,  k = out)
+//   gradient GEMMs (K = the 32 members; the SAME tiles read as MN-major operands -- element (m, f) of a member tile sits at
+//   (m/8) ROW + (f/8) 128 + (m%8) 16 + (f%8) 2, which is at once the canonical K-major layout of [member x feature] and the
+//   canonical MN-major layout of [feature x member]), accumulated in registers over the whole reverse pass (two M = 64 halves):
 //     G1 [128 x 80] += [wt dZ2 | wt dZ1]' [H1 | y0 y1 1 | 0]   ->  dW2, db2 (rows 0..63), dW1, db1 (rows 64..127)
 //     G2 [128 x 16] += [H2 | 1 | 0]' [wt L0, wt L1 | 0]        ->  dW3' (rows 0..63), db3 (row 64)
 //   wt = h b_j is folded into the cotangent side before the bf16 rounding; the backward member GEMM is linear, so the
-//   vector-Jacobian product is recovered by dividing by wt.
+//   vector-Jacobian product is recovered by dividing by wt.  The gradient GEMMs of a stage run asynchronously until the next
+//   stage's H1 is ready to be written.
 //
-// Per adjoint stage: 2 member GEMMs (4 MMAs each) + 2 gradient GEMMs (2 MMAs each); per forward stage: 1 member GEMM.
+// Per adjoint stage: 2 member GEMMs (4 MMAs each) + 2 gradient GEMMs (4 MMAs each); per forward stage: 1 member GEMM.
 // tanh is the hardware tanh.approx.f32 (relative error 2^-11, below the bf16 rounding of the operands).
 // Reference functions replaced: as mlp.cuh (sense functor, split_states, vecjacobian!, ReverseLossCallback).
-// SASS: UTCHMMA (tcgen05.mma), LDTM (tcgen05.ld), UTCBAR (tcgen05.commit).
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include "mlp.cuh"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace b200adj {
 
 constexpr int TC_MEM = 32;                                  // members per CTA
-constexpr int TC_M = 128;                                   // threads per CTA = rows of the member MMAs (4 copies x 32 members)
+constexpr int TC_M = 128;                                   // threads per CTA (one warpgroup)
+constexpr int TC_ROWS = 64;                                 // rows of the member MMAs: 32 members, 32 zero rows
 constexpr int TC_TA_F = 128, TC_TB_F = 80, TC_TC_F = 16;      // feature widths of the tiles
-constexpr uint32_t TC_TMEM_COLS = 256;                      // D: 0..63, G1: 64..143, G2: 144..159
-constexpr uint32_t TC_COL_D = 0, TC_COL_G1 = 64, TC_COL_G2 = 144;
+constexpr int TC_DP = 68;                                   // pitch (floats) of the fp32 accumulator staging tile
 
 struct TcSmem {
-    alignas(128) unsigned char TA[TC_M * TC_TA_F * 2];      // [row][wt dZ2 (64) | wt dZ1 (64)]; dZ2 in all 4 copies, dZ1 in copy 0
+    alignas(128) unsigned char TA[TC_ROWS * TC_TA_F * 2];   // [row][wt dZ2 (64) | wt dZ1 (64)]
     alignas(128) unsigned char TH[TC_MEM * TC_TA_F * 2];    // [member][H2 (64) | 1 | 0 ...]
-    alignas(128) unsigned char TB[TC_M * TC_TB_F * 2];      // [row][H1 (64) | y0 y1 1 | 0 ...]; H1 in all 4 copies
+    alignas(128) unsigned char TB[TC_ROWS * TC_TB_F * 2];   // [row][H1 (64) | y0 y1 1 | 0 ...]
     alignas(128) unsigned char TC[TC_MEM * TC_TC_F * 2];    // [member][wt L0, wt L1 | 0 ...]
     alignas(128) unsigned char W2[64 * 64 * 2];             // (n = out i, k = in j)  = W2[i][j]
     alignas(128) unsigned char W2T[64 * 64 * 2];            // (n = in j,  k = out i) = W2[i][j]
+    alignas(16) float D[TC_MEM * TC_DP];                     // member-GEMM accumulator rows 0..31, fp32
     float W1a[64], W1b[64], b1[64], b2[64], W3a[64], W3b[64], b3[2];
     float red[2][4][TC_MEM][2];                             // per-quarter partial sums of the 2-vectors a stage returns (double-buffered)
-    alignas(8) uint64_t barM, barG;
-    uint32_t tmem;
 };
 
 __device__ __forceinline__ float tanh_fast(float x) { float y; asm("tanh.approx.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 __device__ __forceinline__ uint32_t pack_bf16(float a, float b) { __nv_bfloat162 v = __floats2bfloat162_rn(a, b); return *reinterpret_cast<uint32_t*>(&v); }
-__device__ __forceinline__ constexpr uint32_t tc_idesc(int M, int N, int amn, int bmn) {
-    return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)amn << 15) | ((uint32_t)bmn << 16) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
 // 16-byte chunk kc (features 8 kc .. 8 kc + 7) of row r in a tile of F features
 template <int F> __device__ __forceinline__ uint4* tc_chunk(unsigned char* tile, int r, int kc) {
     return reinterpret_cast<uint4*>(tile + (r >> 3) * (F / 8) * 128 + kc * 128 + (r & 7) * 16);
 }
 
 struct TcState {               // per-thread pipeline bookkeeping (identical in all threads)
-    uint32_t phM = 0, phG = 0, rb = 0;
-    bool gpend = false, gfirst = true;
+    uint32_t rb = 0;
+    bool gpend = false;
 };
+
+// the gradient accumulators G1 (two M = 64 halves x N = 80) and G2 (two halves x N = 16), wgmma fragments
+struct TcGrad {
+    float g1[2][40], g2[2][8];
+    __device__ __forceinline__ void zero() {
+#pragma unroll
+        for (int h = 0; h < 2; h++) {
+#pragma unroll
+            for (int i = 0; i < 40; i++) g1[h][i] = 0.0f;
+#pragma unroll
+            for (int i = 0; i < 8; i++) g2[h][i] = 0.0f;
+        }
+    }
+};
+
+// d = A[64 x 64] B', A = rows 0..63 of a K-major tile (8-row groups a_sbo bytes apart), B = a K-major 64 x 64 weight tile
+__device__ __forceinline__ void tc_member_mma(float (&d)[32], uint32_t a, uint32_t a_sbo, uint32_t b) {
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 4; k++) wgmma_m64n64<0, 0>(d, wgmma_desc(a + k * 256, 128, a_sbo), wgmma_desc(b + k * 256, 128, 1024), k > 0);
+    wgmma_commit();
+    wgmma_wait_all();
+    wgmma_fence_operand(d);
+}
+// the fragment of d (rows row0 + 0..63) into the fp32 staging tile of pitch TC_DP
+__device__ __forceinline__ void tc_stage(float* D, const float (&d)[32], int row0) {
+    const int w = (threadIdx.x >> 5) & 3, l = threadIdx.x & 31, r = row0 + 16 * w + (l >> 2), c = 2 * (l & 3);
+#pragma unroll
+    for (int j = 0; j < 8; j++) {
+        *reinterpret_cast<float2*>(D + r * TC_DP + 8 * j + c) = make_float2(d[4 * j], d[4 * j + 1]);
+        *reinterpret_cast<float2*>(D + (r + 8) * TC_DP + 8 * j + c) = make_float2(d[4 * j + 2], d[4 * j + 3]);
+    }
+}
+// G1 += TA' TB, G2 += TH' TC over the first 16 KS member rows of the tiles (asynchronous: tc_wait_grad before the tiles change)
+template <int KS>
+__device__ __forceinline__ void tc_grad_mma(TcGrad& g, uint32_t TA, uint32_t TB, uint32_t TH, uint32_t TC) {
+    constexpr uint32_t SA = (TC_TA_F / 8) * 128, SB = (TC_TB_F / 8) * 128, SC = (TC_TC_F / 8) * 128;
+    wgmma_fence();
+#pragma unroll
+    for (int h = 0; h < 2; h++)
+#pragma unroll
+        for (int k = 0; k < KS; k++)       // K = 16 members per MMA = 2 member groups of 8
+            wgmma_m64n80<1, 1>(g.g1[h], wgmma_desc(TA + h * 1024 + k * 2 * SA, SA, 128), wgmma_desc(TB + k * 2 * SB, SB, 128), 1u);
+#pragma unroll
+    for (int h = 0; h < 2; h++)
+#pragma unroll
+        for (int k = 0; k < KS; k++)
+            wgmma_m64n16<1, 1>(g.g2[h], wgmma_desc(TH + h * 1024 + k * 2 * SA, SA, 128), wgmma_desc(TC + k * 2 * SC, SC, 128), 1u);
+    wgmma_commit();
+}
+// this CTA's parameter gradient out of the G1 / G2 fragments
+__device__ __forceinline__ void tc_grad_store(TcGrad& g, float* out) {
+    wgmma_wait_all();
+#pragma unroll
+    for (int h = 0; h < 2; h++) { wgmma_fence_operand(g.g1[h]); wgmma_fence_operand(g.g2[h]); }
+    const int w = (threadIdx.x >> 5) & 3, l = threadIdx.x & 31;
+#pragma unroll
+    for (int i = 0; i < 40; i++) {
+        const int r = 16 * w + (l >> 2) + 8 * ((i >> 1) & 1), c = 8 * (i >> 2) + 2 * (l & 3) + (i & 1);
+        if (c < 64) out[MLP_OW2 + c * 64 + r] = g.g1[0][i];      // row i = r: dW2[i][c], db2[i] (c = 66)
+        else if (c == 66) out[MLP_OB2 + r] = g.g1[0][i];
+        if (c == 64) out[MLP_OW1 + r] = g.g1[1][i];               // row 64 + j: dW1[j][c - 64], db1[j] (c = 66)
+        else if (c == 65) out[MLP_OW1 + 64 + r] = g.g1[1][i];
+        else if (c == 66) out[MLP_OB1 + r] = g.g1[1][i];
+    }
+#pragma unroll
+    for (int i = 0; i < 8; i++) {
+        const int r = 16 * w + (l >> 2) + 8 * ((i >> 1) & 1), c = 8 * (i >> 2) + 2 * (l & 3) + (i & 1);
+        if (c < 2) {
+            out[MLP_OW3 + r * 2 + c] = g.g2[0][i];                 // dW3[c][n = r]
+            if (r == 0) out[MLP_OB3 + c] = g.g2[1][i];             // row 64: db3
+        }
+    }
+}
 
 __device__ __forceinline__ void tc_setup(TcSmem& s, const float* p) {
     const int t = threadIdx.x, m = t & 31, w = t >> 5;
@@ -84,31 +153,28 @@ __device__ __forceinline__ void tc_setup(TcSmem& s, const float* p) {
     }
     if (t < 2) s.b3[t] = p[MLP_OB3 + t];
     // constant parts of the tiles: TH features 64.. = [1, 0, ...], TB features 64..79 = 0 (y, 1 written per stage), TC = 0,
-    // TA features 64..127 of the copies 1..3 = 0 (never read by a gradient GEMM, kept finite)
+    // TA / TB rows 32..63 = 0 (the unused rows of the member MMAs)
     const uint4 zero = make_uint4(0, 0, 0, 0);
     *tc_chunk<TC_TA_F>(s.TH, m, 8 + 2 * w) = w == 0 ? make_uint4(0x00003F80u, 0, 0, 0) : zero;       // bf16(1.0) = 0x3F80
     *tc_chunk<TC_TA_F>(s.TH, m, 9 + 2 * w) = zero;
-    *tc_chunk<TC_TB_F>(s.TB, t, 8) = zero;
-    *tc_chunk<TC_TB_F>(s.TB, t, 9) = zero;
-#pragma unroll
-    for (int kc = 8; kc < 16; kc++) *tc_chunk<TC_TA_F>(s.TA, t, kc) = zero;
+    if (w == 0) { *tc_chunk<TC_TB_F>(s.TB, m, 8) = zero; *tc_chunk<TC_TB_F>(s.TB, m, 9) = zero; }
     if (w == 0) { *tc_chunk<TC_TC_F>(s.TC, m, 0) = zero; *tc_chunk<TC_TC_F>(s.TC, m, 1) = zero; }
-    if (w == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&s.tmem)), "r"(TC_TMEM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+    if (w == 2) {
+        const int r = 32 + m;                                                  // rows 32..63
+#pragma unroll
+        for (int kc = 0; kc < TC_TB_F / 8; kc++) *tc_chunk<TC_TB_F>(s.TB, r, kc) = zero;
+#pragma unroll
+        for (int kc = 0; kc < TC_TA_F / 8; kc++) *tc_chunk<TC_TA_F>(s.TA, r, kc) = zero;
     }
-    if (t == 0) { mbar_init(&s.barM, 1); mbar_init(&s.barG, 1); mbar_fence_init(); }
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
 }
 
-__device__ __forceinline__ void tc_wait_grad(TcSmem& s, TcState& st) {
-    if (st.gpend) { mbar_wait(&s.barG, st.phG); st.phG ^= 1; st.gpend = false; asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+__device__ __forceinline__ void tc_wait_grad(TcState& st) {
+    if (st.gpend) { wgmma_wait_all(); st.gpend = false; }
 }
 
-// F = f(y) for this thread's member; leaves H1 (bf16, 4 row copies) in TB and this thread's H2 quarter in registers
+// F = f(y) for this thread's member; leaves H1 (bf16) in TB and this thread's H2 quarter in registers
 template <bool GRAD>
 __device__ __forceinline__ void tc_forward(TcSmem& s, TcState& st, float y0, float y1, float* F, float* H2q) {
     const int t = threadIdx.x, m = t & 31, w = t >> 5;
@@ -120,40 +186,31 @@ __device__ __forceinline__ void tc_forward(TcSmem& s, TcState& st, float y0, flo
         for (int q = 0; q < 8; q++) { const int j = 16 * w + 8 * c + q; h[q] = tanh_fast(fmaf(s.W1a[j], y0, fmaf(s.W1b[j], y1, s.b1[j]))); }
         row[c] = make_uint4(pack_bf16(h[0], h[1]), pack_bf16(h[2], h[3]), pack_bf16(h[4], h[5]), pack_bf16(h[6], h[7]));
     }
-    if (GRAD) tc_wait_grad(s, st);
-#pragma unroll
-    for (int cp = 0; cp < 4; cp++) {
-        *tc_chunk<TC_TB_F>(s.TB, 32 * cp + m, 2 * w) = row[0];
-        *tc_chunk<TC_TB_F>(s.TB, 32 * cp + m, 2 * w + 1) = row[1];
-    }
+    if (GRAD) tc_wait_grad(st);
+    *tc_chunk<TC_TB_F>(s.TB, m, 2 * w) = row[0];
+    *tc_chunk<TC_TB_F>(s.TB, m, 2 * w + 1) = row[1];
     if (GRAD && w == 0) *tc_chunk<TC_TB_F>(s.TB, m, 8) = make_uint4(pack_bf16(y0, y1), pack_bf16(1.0f, 0.0f), 0, 0);
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    if (t == 0) {
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-#pragma unroll
-        for (int k = 0; k < 4; k++)
-            umma_f16(s.tmem + TC_COL_D, umma_smem_desc(smem_u32(s.TB) + k * 256, 128, (TC_TB_F / 8) * 128),
-                     umma_smem_desc(smem_u32(s.W2) + k * 256, 128, 1024), tc_idesc(128, 64, 0, 0), k > 0);
-        umma_commit(&s.barM);
-    }
-    mbar_wait(&s.barM, st.phM); st.phM ^= 1;
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    float f0 = 0.0f, f1 = 0.0f;
     {
-        uint32_t r[16];
-        tmem_ld16(s.tmem + ((uint32_t)(w * 32) << 16) + TC_COL_D + 16 * w, r);       // copy w of member m, columns 16 w ..
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+        float d[32];
+        tc_member_mma(d, smem_u32(s.TB), (TC_TB_F / 8) * 128, smem_u32(s.W2));
+        if (w < 2) tc_stage(s.D, d, 0);
+    }
+    __syncthreads();
+    float f0 = 0.0f, f1 = 0.0f;
 #pragma unroll
-        for (int q = 0; q < 16; q++) {
-            const int n = 16 * w + q;
-            const float h2 = tanh_fast(__uint_as_float(r[q]) + s.b2[n]);
+    for (int q4 = 0; q4 < 4; q4++) {
+        const float4 z = *reinterpret_cast<const float4*>(s.D + m * TC_DP + 16 * w + 4 * q4);     // member m, columns 16 w ..
+        const float zz[4] = {z.x, z.y, z.z, z.w};
+#pragma unroll
+        for (int e = 0; e < 4; e++) {
+            const int q = 4 * q4 + e, n = 16 * w + q;
+            const float h2 = tanh_fast(zz[e] + s.b2[n]);
             H2q[q] = h2;
             f0 = fmaf(s.W3a[n], h2, f0); f1 = fmaf(s.W3b[n], h2, f1);
         }
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     // sum over the four feature quarters (fixed order => all four threads of a member hold the same bits)
     float (*red)[TC_MEM][2] = s.red[st.rb]; st.rb ^= 1;
     red[w][m][0] = f0; red[w][m][1] = f1;
@@ -165,7 +222,7 @@ __device__ __forceinline__ void tc_forward(TcSmem& s, TcState& st, float y0, flo
 // J = (df/dy)' L at the point of the last tc_forward; issues the gradient GEMMs with weight wt (members with valid = false
 // contribute nothing)
 template <bool GRAD = true>
-__device__ __forceinline__ void tc_backward(TcSmem& s, TcState& st, float wt, float L0, float L1, bool valid, const float* H2q, float* J) {
+__device__ __forceinline__ void tc_backward(TcSmem& s, TcState& st, TcGrad& g, float wt, float L0, float L1, bool valid, const float* H2q, float* J) {
     const int t = threadIdx.x, m = t & 31, w = t >> 5;
     const float wv = valid ? wt : 0.0f;
     uint4 dzc[2], hhc[2];
@@ -181,42 +238,34 @@ __device__ __forceinline__ void tc_backward(TcSmem& s, TcState& st, float wt, fl
         dzc[c] = make_uint4(pack_bf16(dz[0], dz[1]), pack_bf16(dz[2], dz[3]), pack_bf16(dz[4], dz[5]), pack_bf16(dz[6], dz[7]));
         hhc[c] = make_uint4(pack_bf16(hh[0], hh[1]), pack_bf16(hh[2], hh[3]), pack_bf16(hh[4], hh[5]), pack_bf16(hh[6], hh[7]));
     }
-#pragma unroll
-    for (int cp = 0; cp < 4; cp++) {
-        *tc_chunk<TC_TA_F>(s.TA, 32 * cp + m, 2 * w) = dzc[0];
-        *tc_chunk<TC_TA_F>(s.TA, 32 * cp + m, 2 * w + 1) = dzc[1];
-    }
+    *tc_chunk<TC_TA_F>(s.TA, m, 2 * w) = dzc[0];
+    *tc_chunk<TC_TA_F>(s.TA, m, 2 * w + 1) = dzc[1];
     *tc_chunk<TC_TA_F>(s.TH, m, 2 * w) = hhc[0];
     *tc_chunk<TC_TA_F>(s.TH, m, 2 * w + 1) = hhc[1];
     if (w == 0) *tc_chunk<TC_TC_F>(s.TC, m, 0) = make_uint4(pack_bf16(wv * L0, wv * L1), 0, 0, 0);
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    if (t == 0) {
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-#pragma unroll
-        for (int k = 0; k < 4; k++)
-            umma_f16(s.tmem + TC_COL_D, umma_smem_desc(smem_u32(s.TA) + k * 256, 128, (TC_TA_F / 8) * 128),
-                     umma_smem_desc(smem_u32(s.W2T) + k * 256, 128, 1024), tc_idesc(128, 64, 0, 0), k > 0);
-        umma_commit(&s.barM);
+    {
+        float d[32];
+        tc_member_mma(d, smem_u32(s.TA), (TC_TA_F / 8) * 128, smem_u32(s.W2T));
+        if (w < 2) tc_stage(s.D, d, 0);
     }
-    mbar_wait(&s.barM, st.phM); st.phM ^= 1;
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+    __syncthreads();
     float j0 = 0.0f, j1 = 0.0f;
     {
-        uint32_t r[16];
-        tmem_ld16(s.tmem + ((uint32_t)(w * 32) << 16) + TC_COL_D + 16 * w, r);
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
         float dz1[16];
 #pragma unroll
         for (int c = 0; c < 2; c++) {
             const uint4 hv = *tc_chunk<TC_TB_F>(s.TB, m, 2 * w + c);      // this member's H1 (bf16), features 16 w + 8 c ..
             const uint32_t hw[4] = {hv.x, hv.y, hv.z, hv.w};
+            const float4 z0 = *reinterpret_cast<const float4*>(s.D + m * TC_DP + 16 * w + 8 * c);
+            const float4 z1 = *reinterpret_cast<const float4*>(s.D + m * TC_DP + 16 * w + 8 * c + 4);
+            const float zz[8] = {z0.x, z0.y, z0.z, z0.w, z1.x, z1.y, z1.z, z1.w};
 #pragma unroll
             for (int q = 0; q < 8; q++) {
                 const int j = 16 * w + 8 * c + q;
                 const float h1 = __uint_as_float((q & 1) ? (hw[q >> 1] & 0xFFFF0000u) : (hw[q >> 1] << 16));
-                const float d = __uint_as_float(r[8 * c + q]) * (1.0f - h1 * h1);      // wt dZ1
+                const float d = zz[q] * (1.0f - h1 * h1);      // wt dZ1
                 dz1[8 * c + q] = d;
                 j0 = fmaf(s.W1a[j], d, j0); j1 = fmaf(s.W1b[j], d, j1);
             }
@@ -227,31 +276,11 @@ __device__ __forceinline__ void tc_backward(TcSmem& s, TcState& st, float wt, fl
     float (*red)[TC_MEM][2] = s.red[st.rb]; st.rb ^= 1;
     red[w][m][0] = j0; red[w][m][1] = j1;
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
     const float inv = 1.0f / wt;
     J[0] = ((red[0][m][0] + red[1][m][0]) + (red[2][m][0] + red[3][m][0])) * inv;
     J[1] = ((red[0][m][1] + red[1][m][1]) + (red[2][m][1] + red[3][m][1])) * inv;
-    if (GRAD && t == 0) {
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t acc0 = st.gfirst ? 0u : 1u;
-#pragma unroll
-        for (int k = 0; k < TC_MEM / 16; k++)        // K = 16 members per MMA = 2 member groups of 8; the 32 members of copy 0
-            umma_f16(s.tmem + TC_COL_G1, umma_smem_desc(smem_u32(s.TA) + k * 2 * (TC_TA_F / 8) * 128, (TC_TA_F / 8) * 128, 128),
-                     umma_smem_desc(smem_u32(s.TB) + k * 2 * (TC_TB_F / 8) * 128, (TC_TB_F / 8) * 128, 128), tc_idesc(128, TC_TB_F, 1, 1), (k > 0) ? 1u : acc0);
-#pragma unroll
-        for (int k = 0; k < TC_MEM / 16; k++)
-            umma_f16(s.tmem + TC_COL_G2, umma_smem_desc(smem_u32(s.TH) + k * 2 * (TC_TA_F / 8) * 128, (TC_TA_F / 8) * 128, 128),
-                     umma_smem_desc(smem_u32(s.TC) + k * 2 * (TC_TC_F / 8) * 128, (TC_TC_F / 8) * 128, 128), tc_idesc(128, TC_TC_F, 1, 1), (k > 0) ? 1u : acc0);
-        umma_commit(&s.barG);
-    }
-    if (GRAD) { st.gfirst = false; st.gpend = true; }
-}
-
-__device__ __forceinline__ void tc_teardown(TcSmem& s) {
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if ((threadIdx.x >> 5) == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(s.tmem), "r"(TC_TMEM_COLS) : "memory");
+    if (GRAD) { tc_grad_mma<TC_MEM / 16>(g, smem_u32(s.TA), smem_u32(s.TB), smem_u32(s.TH), smem_u32(s.TC)); st.gpend = true; }
 }
 
 // ---- forward ensemble solve (fixed-step Tsit5) ----
@@ -300,12 +329,11 @@ __global__ void __launch_bounds__(TC_M) mlp_tc_forward_kernel(const __grid_const
         }
     }
     if (writer && a.status) a.status[col] = (isfinite(u[0]) && isfinite(u[1])) ? 0 : 1;
-    tc_teardown(s);
 }
 
 // ---- fused reverse pass (same stage sequence as mlp_reverse_kernel): InterpolatingAdjoint, or GaussAdjoint (GAUSS: seven
 // adjoint stages without gradient GEMMs, then the gradient GEMMs at the three Gauss-Legendre nodes of the step, weight (h/2) w_g,
-// accumulated in the same TMEM tiles) ----
+// accumulated in the same registers) ----
 template <int COST, bool GAUSS = false>
 __global__ void __launch_bounds__(TC_M) mlp_tc_reverse_kernel(const __grid_constant__ MlpArgs<float> a) {
     extern __shared__ __align__(128) unsigned char tc_smem_raw[];
@@ -317,6 +345,8 @@ __global__ void __launch_bounds__(TC_M) mlp_tc_reverse_kernel(const __grid_const
     const Tsit5Tables& tb = a.tb;
     tc_setup(s, a.p);
     TcState st;
+    TcGrad g;
+    g.zero();
     float lam[2] = {0.0f, 0.0f}, uhi[2], ulo[2], kf[7][2], ka[7][2], H2q[16], F[2], J[2];
     auto cotangent = [&](int ks, const float* yy) {
         if (COST == COST_EXPLICIT) { lam[0] += a.dLdu[((int64_t)ks * 2) * N + col]; lam[1] += a.dLdu[((int64_t)ks * 2 + 1) * N + col]; }
@@ -362,8 +392,8 @@ __global__ void __launch_bounds__(TC_M) mlp_tc_reverse_kernel(const __grid_const
                 y[c] = (float)yv;
             }
             tc_forward<true>(s, st, y[0], y[1], F, H2q);
-            if (GAUSS) tc_backward<false>(s, st, 1.0f, L[0], L[1], live, H2q, J);
-            else tc_backward<true>(s, st, (float)tb.hA[6][sg], L[0], L[1], live, H2q, J);
+            if (GAUSS) tc_backward<false>(s, st, g, 1.0f, L[0], L[1], live, H2q, J);
+            else tc_backward<true>(s, st, g, (float)tb.hA[6][sg], L[0], L[1], live, H2q, J);
             ka[sg][0] = J[0]; ka[sg][1] = J[1];
         }
         if (GAUSS) {
@@ -377,7 +407,7 @@ __global__ void __launch_bounds__(TC_M) mlp_tc_reverse_kernel(const __grid_const
                     L[c] = (float)l; y[c] = (float)yv;
                 }
                 tc_forward<true>(s, st, y[0], y[1], F, H2q);
-                tc_backward<true>(s, st, (float)tb.hGW[gq], L[0], L[1], live, H2q, J);
+                tc_backward<true>(s, st, g, (float)tb.hGW[gq], L[0], L[1], live, H2q, J);
             }
         }
 #pragma unroll
@@ -391,40 +421,8 @@ __global__ void __launch_bounds__(TC_M) mlp_tc_reverse_kernel(const __grid_const
         if (!a.kst) { kf[6][0] = kf[0][0]; kf[6][1] = kf[0][1]; }
     }
     if (writer) { a.du0[col] = lam[0]; a.du0[N + col] = lam[1]; }
-    // ---- parameter gradient of this CTA out of TMEM: thread t = row t of G1 / G2 ----
-    tc_wait_grad(s, st);
-    float* out = a.partials + (int64_t)blockIdx.x * MLP_P;
-    const uint32_t lane_base = s.tmem + ((uint32_t)((t >> 5) * 32) << 16);
-    const bool any = a.S > 0;
-#pragma unroll 1
-    for (int cb = 0; cb < TC_TB_F; cb += 16) {
-        uint32_t r[16];
-        tmem_ld16(lane_base + TC_COL_G1 + cb, r);
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-        for (int q = 0; q < 16; q++) {
-            const int g = cb + q;
-            const float v = any ? __uint_as_float(r[q]) : 0.0f;
-            if (t < 64) {                    // row i = t: dW2[i][g] (g < 64), db2[i] (g = 66)
-                if (g < 64) out[MLP_OW2 + g * 64 + t] = v;
-                else if (g == 66) out[MLP_OB2 + t] = v;
-            } else {                         // row 64 + j: dW1[j][c] (g = 64 + c), db1[j] (g = 66)
-                const int j = t - 64;
-                if (g == 64) out[MLP_OW1 + j] = v;
-                else if (g == 65) out[MLP_OW1 + 64 + j] = v;
-                else if (g == 66) out[MLP_OB1 + j] = v;
-            }
-        }
-    }
-    {
-        uint32_t r[16];
-        tmem_ld16(lane_base + TC_COL_G2, r);
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        const float v0 = any ? __uint_as_float(r[0]) : 0.0f, v1 = any ? __uint_as_float(r[1]) : 0.0f;
-        if (t < 64) { out[MLP_OW3 + t * 2] = v0; out[MLP_OW3 + t * 2 + 1] = v1; }      // dW3[c][n = t]
-        else if (t == 64) { out[MLP_OB3] = v0; out[MLP_OB3 + 1] = v1; }
-    }
-    tc_teardown(s);
+    // ---- parameter gradient of this CTA out of the accumulator fragments ----
+    tc_grad_store(g, a.partials + (int64_t)blockIdx.x * MLP_P);
 }
 
 }  // namespace b200adj

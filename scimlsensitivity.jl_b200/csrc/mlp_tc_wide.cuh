@@ -1,7 +1,7 @@
 // mlp_tc_wide.cuh -- the WIDE layout of the tensor-core neural-ODE kernels (mlp_tc.cuh): one CTA = 128 ensemble members = the
-// 128 rows (TMEM lanes) of every MMA, one thread per member (64 tanh per layer and thread).  Highest throughput once every SM
-// has work (N >= 2 x 148 x 32 members); below that the 32-member layout of mlp_tc.cuh has 4x more CTAs and shorter stages.
-// The GEMMs, tiles and descriptors are those of mlp_tc.cuh (all 128 rows are distinct members here).
+// 128 rows (two M = 64 halves) of every MMA, one thread per member (64 tanh per layer and thread).  Highest throughput once
+// every SM has work (N >= 2 x n_SM x 32 members); below that the 32-member layout of mlp_tc.cuh has 4x more CTAs and shorter
+// stages.  The GEMMs, tiles and descriptors are those of mlp_tc.cuh (all 128 rows are distinct members here).
 #pragma once
 #include "mlp_tc.cuh"
 
@@ -16,14 +16,12 @@ struct TcwSmem {
     alignas(128) unsigned char TC[TCW_M * TC_TC_F * 2];      // [member][wt L0, wt L1 | 0 ...]
     alignas(128) unsigned char W2[64 * 64 * 2];             // (n = out i, k = in j)  = W2[i][j]
     alignas(128) unsigned char W2T[64 * 64 * 2];            // (n = in j,  k = out i) = W2[i][j]
+    alignas(16) float D[TCW_M * TC_DP];                      // member-GEMM accumulator, fp32
     float W1a[64], W1b[64], b1[64], b2[64], W3a[64], W3b[64], b3[2];
-    alignas(8) uint64_t barM, barG;
-    uint32_t tmem;
 };
 
 struct TcwState {               // per-thread pipeline bookkeeping (identical in all threads)
-    uint32_t phM = 0, phG = 0;
-    bool gpend = false, gfirst = true;
+    bool gpend = false;
 };
 
 __device__ __forceinline__ void tcw_setup(TcwSmem& s, const float* p) {
@@ -48,19 +46,22 @@ __device__ __forceinline__ void tcw_setup(TcwSmem& s, const float* p) {
     *tc_chunk<TC_TB_F>(s.TB, t, 9) = zero;
     *tc_chunk<TC_TC_F>(s.TC, t, 0) = zero;
     *tc_chunk<TC_TC_F>(s.TC, t, 1) = zero;
-    if ((t >> 5) == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&s.tmem)), "r"(TC_TMEM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    if (t == 0) { mbar_init(&s.barM, 1); mbar_init(&s.barG, 1); mbar_fence_init(); }
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
 }
 
-__device__ __forceinline__ void tcw_wait_grad(TcwSmem& s, TcwState& st) {
-    if (st.gpend) { mbar_wait(&s.barG, st.phG); st.phG ^= 1; st.gpend = false; asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+__device__ __forceinline__ void tcw_wait_grad(TcwState& st) {
+    if (st.gpend) { wgmma_wait_all(); st.gpend = false; }
+}
+
+// the member GEMM of this stage (A = the K-major tile a of 128 rows) staged to s.D as fp32, one M = 64 half at a time
+__device__ __forceinline__ void tcw_member_mma(TcwSmem& s, const unsigned char* a, uint32_t a_sbo, const unsigned char* b) {
+#pragma unroll 1
+    for (int h = 0; h < 2; h++) {
+        float d[32];
+        tc_member_mma(d, smem_u32(a) + h * 8 * a_sbo, a_sbo, smem_u32(b));
+        tc_stage(s.D, d, 64 * h);
+    }
 }
 
 // F = f(y); leaves H1 (bf16) in this member's TB row and H2 in registers
@@ -75,46 +76,34 @@ __device__ __forceinline__ void tcw_forward(TcwSmem& s, TcwState& st, float y0, 
         for (int q = 0; q < 8; q++) { const int j = kc * 8 + q; h[q] = tanh_fast(fmaf(s.W1a[j], y0, fmaf(s.W1b[j], y1, s.b1[j]))); }
         row[kc] = make_uint4(pack_bf16(h[0], h[1]), pack_bf16(h[2], h[3]), pack_bf16(h[4], h[5]), pack_bf16(h[6], h[7]));
     }
-    if (GRAD) tcw_wait_grad(s, st);
+    if (GRAD) tcw_wait_grad(st);
 #pragma unroll
     for (int kc = 0; kc < 8; kc++) *tc_chunk<TC_TB_F>(s.TB, t, kc) = row[kc];
     if (GRAD) *tc_chunk<TC_TB_F>(s.TB, t, 8) = make_uint4(pack_bf16(y0, y1), pack_bf16(1.0f, 0.0f), 0, 0);
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    if (t == 0) {
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-#pragma unroll
-        for (int k = 0; k < 4; k++)
-            umma_f16(s.tmem + TC_COL_D, umma_smem_desc(smem_u32(s.TB) + k * 256, 128, (TC_TB_F / 8) * 128),
-                     umma_smem_desc(smem_u32(s.W2) + k * 256, 128, 1024), tc_idesc(128, 64, 0, 0), k > 0);
-        umma_commit(&s.barM);
-    }
-    mbar_wait(&s.barM, st.phM); st.phM ^= 1;
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+    tcw_member_mma(s, s.TB, (TC_TB_F / 8) * 128, s.W2);
+    __syncthreads();
     float f0 = s.b3[0], f1 = s.b3[1];
-    const uint32_t lane_base = s.tmem + ((uint32_t)((t >> 5) * 32) << 16) + TC_COL_D;
 #pragma unroll
-    for (int cb = 0; cb < 64; cb += 16) {
-        uint32_t r[16];
-        tmem_ld16(lane_base + cb, r);
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+    for (int q4 = 0; q4 < 16; q4++) {
+        const float4 z = *reinterpret_cast<const float4*>(s.D + t * TC_DP + 4 * q4);
+        const float zz[4] = {z.x, z.y, z.z, z.w};
 #pragma unroll
-        for (int q = 0; q < 16; q++) {
-            const int n = cb + q;
-            const float h2 = tanh_fast(__uint_as_float(r[q]) + s.b2[n]);
+        for (int e = 0; e < 4; e++) {
+            const int n = 4 * q4 + e;
+            const float h2 = tanh_fast(zz[e] + s.b2[n]);
             H2[n] = h2;
             f0 = fmaf(s.W3a[n], h2, f0); f1 = fmaf(s.W3b[n], h2, f1);
         }
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     F[0] = f0; F[1] = f1;
 }
 
 // J = (df/dy)' L at the point of the last tcw_forward; issues the gradient GEMMs with weight wt (members with valid = false
 // contribute nothing)
 template <bool GRAD = true>
-__device__ __forceinline__ void tcw_backward(TcwSmem& s, TcwState& st, float wt, float L0, float L1, bool valid, const float* H2, float* J) {
+__device__ __forceinline__ void tcw_backward(TcwSmem& s, TcwState& st, TcGrad& g, float wt, float L0, float L1, bool valid, const float* H2, float* J) {
     const int t = threadIdx.x;
     const float wv = valid ? wt : 0.0f;
 #pragma unroll
@@ -131,35 +120,25 @@ __device__ __forceinline__ void tcw_backward(TcwSmem& s, TcwState& st, float wt,
     }
     *tc_chunk<TC_TC_F>(s.TC, t, 0) = make_uint4(pack_bf16(wv * L0, wv * L1), 0, 0, 0);
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    if (t == 0) {
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-#pragma unroll
-        for (int k = 0; k < 4; k++)
-            umma_f16(s.tmem + TC_COL_D, umma_smem_desc(smem_u32(s.TA) + k * 256, 128, (TC_TA_F / 8) * 128),
-                     umma_smem_desc(smem_u32(s.W2T) + k * 256, 128, 1024), tc_idesc(128, 64, 0, 0), k > 0);
-        umma_commit(&s.barM);
-    }
-    mbar_wait(&s.barM, st.phM); st.phM ^= 1;
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+    tcw_member_mma(s, s.TA, (TC_TA_F / 8) * 128, s.W2T);
+    __syncthreads();
     float j0 = 0.0f, j1 = 0.0f;
-    const uint32_t lane_base = s.tmem + ((uint32_t)((t >> 5) * 32) << 16) + TC_COL_D;
 #pragma unroll
     for (int cb = 0; cb < 64; cb += 16) {
-        uint32_t r[16];
-        tmem_ld16(lane_base + cb, r);
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
         float dz1[16];
 #pragma unroll
         for (int half = 0; half < 2; half++) {
             const uint4 hv = *tc_chunk<TC_TB_F>(s.TB, t, cb / 8 + half);      // this member's H1 (bf16), features cb + 8 half ..
             const uint32_t hw[4] = {hv.x, hv.y, hv.z, hv.w};
+            const float4 z0 = *reinterpret_cast<const float4*>(s.D + t * TC_DP + cb + 8 * half);
+            const float4 z1 = *reinterpret_cast<const float4*>(s.D + t * TC_DP + cb + 8 * half + 4);
+            const float zz[8] = {z0.x, z0.y, z0.z, z0.w, z1.x, z1.y, z1.z, z1.w};
 #pragma unroll
             for (int q = 0; q < 8; q++) {
                 const int j = cb + half * 8 + q;
                 const float h1 = __uint_as_float((q & 1) ? (hw[q >> 1] & 0xFFFF0000u) : (hw[q >> 1] << 16));
-                const float d = __uint_as_float(r[half * 8 + q]) * (1.0f - h1 * h1);      // wt dZ1
+                const float d = zz[q] * (1.0f - h1 * h1);      // wt dZ1
                 dz1[half * 8 + q] = d;
                 j0 = fmaf(s.W1a[j], d, j0); j1 = fmaf(s.W1b[j], d, j1);
             }
@@ -170,28 +149,8 @@ __device__ __forceinline__ void tcw_backward(TcwSmem& s, TcwState& st, float wt,
     const float inv = 1.0f / wt;
     J[0] = j0 * inv; J[1] = j1 * inv;
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    if (GRAD && t == 0) {
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t acc0 = st.gfirst ? 0u : 1u;
-#pragma unroll
-        for (int k = 0; k < 8; k++)        // K = 16 members per MMA = 2 member groups of 8
-            umma_f16(s.tmem + TC_COL_G1, umma_smem_desc(smem_u32(s.TA) + k * 2 * (TC_TA_F / 8) * 128, (TC_TA_F / 8) * 128, 128),
-                     umma_smem_desc(smem_u32(s.TB) + k * 2 * (TC_TB_F / 8) * 128, (TC_TB_F / 8) * 128, 128), tc_idesc(128, TC_TB_F, 1, 1), (k > 0) ? 1u : acc0);
-#pragma unroll
-        for (int k = 0; k < 8; k++)
-            umma_f16(s.tmem + TC_COL_G2, umma_smem_desc(smem_u32(s.TH) + k * 2 * (TC_TA_F / 8) * 128, (TC_TA_F / 8) * 128, 128),
-                     umma_smem_desc(smem_u32(s.TC) + k * 2 * (TC_TC_F / 8) * 128, (TC_TC_F / 8) * 128, 128), tc_idesc(128, TC_TC_F, 1, 1), (k > 0) ? 1u : acc0);
-        umma_commit(&s.barG);
-    }
-    if (GRAD) { st.gfirst = false; st.gpend = true; }
-}
-
-__device__ __forceinline__ void tcw_teardown(TcwSmem& s) {
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if ((threadIdx.x >> 5) == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(s.tmem), "r"(TC_TMEM_COLS) : "memory");
+    if (GRAD) { tc_grad_mma<TCW_M / 16>(g, smem_u32(s.TA), smem_u32(s.TB), smem_u32(s.TH), smem_u32(s.TC)); st.gpend = true; }
 }
 
 // ---- forward ensemble solve (fixed-step Tsit5) ----
@@ -240,12 +199,11 @@ __global__ void __launch_bounds__(TCW_M) mlp_tcw_forward_kernel(const __grid_con
         }
     }
     if (live && a.status) a.status[col] = (isfinite(u[0]) && isfinite(u[1])) ? 0 : 1;
-    tcw_teardown(s);
 }
 
 // ---- fused reverse pass (same stage sequence as mlp_reverse_kernel): InterpolatingAdjoint, or GaussAdjoint (GAUSS: seven
 // adjoint stages without gradient GEMMs, then the gradient GEMMs at the three Gauss-Legendre nodes of the step, weight (h/2) w_g,
-// accumulated in the same TMEM tiles) ----
+// accumulated in the same registers) ----
 template <int COST, bool GAUSS = false>
 __global__ void __launch_bounds__(TCW_M) mlp_tcw_reverse_kernel(const __grid_constant__ MlpArgs<float> a) {
     extern __shared__ __align__(128) unsigned char tcw_smem_raw[];
@@ -257,6 +215,8 @@ __global__ void __launch_bounds__(TCW_M) mlp_tcw_reverse_kernel(const __grid_con
     const Tsit5Tables& tb = a.tb;
     tcw_setup(s, a.p);
     TcwState st;
+    TcGrad g;
+    g.zero();
     float lam[2] = {0.0f, 0.0f}, uhi[2], ulo[2], kf[7][2], ka[7][2], H2[64], F[2], J[2];
     auto cotangent = [&](int ks, const float* yy) {
         if (COST == COST_EXPLICIT) { lam[0] += a.dLdu[((int64_t)ks * 2) * N + col]; lam[1] += a.dLdu[((int64_t)ks * 2 + 1) * N + col]; }
@@ -302,8 +262,8 @@ __global__ void __launch_bounds__(TCW_M) mlp_tcw_reverse_kernel(const __grid_con
                 y[c] = (float)yv;
             }
             tcw_forward<true>(s, st, y[0], y[1], F, H2);
-            if (GAUSS) tcw_backward<false>(s, st, 1.0f, L[0], L[1], live, H2, J);
-            else tcw_backward<true>(s, st, (float)tb.hA[6][sg], L[0], L[1], live, H2, J);
+            if (GAUSS) tcw_backward<false>(s, st, g, 1.0f, L[0], L[1], live, H2, J);
+            else tcw_backward<true>(s, st, g, (float)tb.hA[6][sg], L[0], L[1], live, H2, J);
             ka[sg][0] = J[0]; ka[sg][1] = J[1];
         }
         if (GAUSS) {
@@ -317,7 +277,7 @@ __global__ void __launch_bounds__(TCW_M) mlp_tcw_reverse_kernel(const __grid_con
                     L[c] = (float)l; y[c] = (float)yv;
                 }
                 tcw_forward<true>(s, st, y[0], y[1], F, H2);
-                tcw_backward<true>(s, st, (float)tb.hGW[gq], L[0], L[1], live, H2, J);
+                tcw_backward<true>(s, st, g, (float)tb.hGW[gq], L[0], L[1], live, H2, J);
             }
         }
 #pragma unroll
@@ -331,40 +291,8 @@ __global__ void __launch_bounds__(TCW_M) mlp_tcw_reverse_kernel(const __grid_con
         if (!a.kst) { kf[6][0] = kf[0][0]; kf[6][1] = kf[0][1]; }
     }
     if (live) { a.du0[col] = lam[0]; a.du0[N + col] = lam[1]; }
-    // ---- parameter gradient of this CTA out of TMEM: thread t = row t of G1 / G2 ----
-    tcw_wait_grad(s, st);
-    float* out = a.partials + (int64_t)blockIdx.x * MLP_P;
-    const uint32_t lane_base = s.tmem + ((uint32_t)((t >> 5) * 32) << 16);
-    const bool any = a.S > 0;
-#pragma unroll 1
-    for (int cb = 0; cb < TC_TB_F; cb += 16) {
-        uint32_t r[16];
-        tmem_ld16(lane_base + TC_COL_G1 + cb, r);
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-        for (int q = 0; q < 16; q++) {
-            const int g = cb + q;
-            const float v = any ? __uint_as_float(r[q]) : 0.0f;
-            if (t < 64) {                    // row i = t: dW2[i][g] (g < 64), db2[i] (g = 66)
-                if (g < 64) out[MLP_OW2 + g * 64 + t] = v;
-                else if (g == 66) out[MLP_OB2 + t] = v;
-            } else {                         // row 64 + j: dW1[j][c] (g = 64 + c), db1[j] (g = 66)
-                const int j = t - 64;
-                if (g == 64) out[MLP_OW1 + j] = v;
-                else if (g == 65) out[MLP_OW1 + 64 + j] = v;
-                else if (g == 66) out[MLP_OB1 + j] = v;
-            }
-        }
-    }
-    {
-        uint32_t r[16];
-        tmem_ld16(lane_base + TC_COL_G2, r);
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        const float v0 = any ? __uint_as_float(r[0]) : 0.0f, v1 = any ? __uint_as_float(r[1]) : 0.0f;
-        if (t < 64) { out[MLP_OW3 + t * 2] = v0; out[MLP_OW3 + t * 2 + 1] = v1; }      // dW3[c][n = t]
-        else if (t == 64) { out[MLP_OB3] = v0; out[MLP_OB3 + 1] = v1; }
-    }
-    tcw_teardown(s);
+    // ---- parameter gradient of this CTA out of the accumulator fragments ----
+    tc_grad_store(g, a.partials + (int64_t)blockIdx.x * MLP_P);
 }
 
 }  // namespace b200adj

@@ -188,8 +188,8 @@ __global__ void __launch_bounds__(512) tsit5_forward_kernel(const __grid_constan
     store_state<D>(a.ckpt, a.Npad, gi, u);
     if (active && a.saved) { int ks = a.save_of_step[0]; if (ks >= 0) store_state<D>(a.saved + (int64_t)ks * stride, a.N, i, u); }
     Fam::f(u, p, k[0]);
-    // (travelling warp groups as in the reverse kernel were tried here: the rotation itself gains 3%, the extra control
-    // flow costs the free-running loop 8% -- profiles/r1_tuning_log.md -- so the forward kernel launches `slots` threads)
+    // (travelling warp groups as in the reverse kernel were tried here: the extra control flow of the free-running loop
+    // costs more than the rotation gains, so the forward kernel launches `slots` threads)
     for (int n = 0; n < a.S; n++) {
         tsit5_stage<D, 1>(a.tb, u, k, tmp); Fam::f(tmp, p, k[1]);
         tsit5_stage<D, 2>(a.tb, u, k, tmp); Fam::f(tmp, p, k[2]);
@@ -329,8 +329,8 @@ __device__ __forceinline__ void add_cotangent(const Args& a, int ks, int64_t str
 
 // ------------------------------------------------------------------------------------------------------------
 // Fused reverse pass.  SA in {SA_INTERP, SA_GAUSS, SA_BACKSOLVE}.
-// Register cap: 65536 members / 148 SMs = 443 threads per SM must be resident at once, otherwise a second, nearly
-// empty wave doubles the kernel time (every thread runs the full time loop): 448 threads/SM => <= 144 registers.
+// Register cap: 65536 members / 132 SMs (H100 SXM) = 497 threads per SM must be resident at once, otherwise a second,
+// nearly empty wave doubles the kernel time (every thread runs the full time loop): 512 threads/SM => <= 128 registers.
 // ------------------------------------------------------------------------------------------------------------
 #ifndef B200_REV_MAXREG
 #define B200_REV_MAXREG 128
@@ -347,9 +347,8 @@ template <class Fam, int SA, bool SHARED_P, int COST, bool CONT, class R = doubl
 __global__ void __maxnreg__(B200_REV_MAXREG) tsit5_reverse_kernel(const __grid_constant__ OdeRevArgsT<R> a) {
     constexpr int D = Fam::D, P = Fam::P;
     // BLOCK = member slots of this block.  When the slot count is not a multiple of 4 warps the SM's four sub-partitions
-    // (one fp64 pipe each; warp w lives on sub-partition w % 4 -- tuning/smsp_map.cu) would carry unequal warp counts for
-    // the whole solve: 448 slots = 4,4,3,3 warps, and the kernel runs at the pace of the 4-warp sub-partitions (measured:
-    // 448 and 512 slots take the same 2.02 ms, 384 slots 1.58 ms).  The host then launches whole warp rows
+    // (one fp64 pipe each; warp w lives on sub-partition w % 4) would carry unequal warp counts for the whole solve:
+    // 448 slots = 4,4,3,3 warps, and the kernel runs at the pace of the 4-warp sub-partitions.  The host then launches whole warp rows
     // (blockDim.x = 128 * ceil(BLOCK / 128)) and the rw = (BLOCK / 32) % 4 warp groups of the top row travel round the
     // four sub-partitions, one hop per time step: group q4+e is advanced through step c by warp q4 + ((e + c) & 3), which
     // takes the group's live state from its predecessor through shared memory (producer/consumer named barriers) and

@@ -2,7 +2,7 @@
 """Summarise `nvcc -Xptxas -v` output: kernel (demangled) -> registers / spills / smem."""
 import re, subprocess, sys
 txt = open(sys.argv[1]).read()
-pat = re.compile(r"Compiling entry function '([^']+)' for 'sm_100a'\n.*\n\s+(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads\n.*?Used (\d+) registers(.*)")
+pat = re.compile(r"Compiling entry function '([^']+)' for 'sm_90a'\n.*\n\s+(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads\n.*?Used (\d+) registers(.*)")
 names = [m.group(1) for m in pat.finditer(txt)]
 dem = subprocess.run(["c++filt"] + names, capture_output=True, text=True).stdout.splitlines() if names else []
 flt = sys.argv[2] if len(sys.argv) > 2 else ""

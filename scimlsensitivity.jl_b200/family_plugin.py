@@ -32,7 +32,7 @@ def build_family_plugin(header, struct, name, out=None, has_jac=False, verbose=F
             if has_jac:
                 f.write("#define B200ADJ_FAMILY_HAS_JAC 1\n")
             f.write('#include "family_plugin.inc"\n')
-        cmd = [_lib.nvcc_path(), "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC",
+        cmd = [_lib.nvcc_path(), "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC",
                "-shared", "-I", _lib._CSRC, src, "-o", out, "-L", pkg, "-l:" + os.path.basename(_lib.LIB_PATH), "-Xlinker", "-rpath", "-Xlinker", pkg]
         res = subprocess.run(cmd, capture_output=True, text=True)
         if res.returncode != 0:

@@ -48,7 +48,7 @@ class ReactantVJP(VJPChoice):
 
 @dataclass(frozen=True)
 class B200VJP(VJPChoice):
-    """Hand-differentiated sm_100a device VJP for a named RHS family (csrc/families.cuh)."""
+    """Hand-differentiated sm_90a device VJP for a named RHS family (csrc/families.cuh)."""
     pass
 
 

@@ -62,14 +62,14 @@ BLOCKS = {"W1": slice(0, 2 * H), "b1": slice(2 * H, 3 * H), "W2": slice(3 * H, 3
 @pytest.mark.parametrize("sensealg", ["interpolating", "gauss"])
 def test_mlp_bf16_tensor_core_path(N, cost, sensealg):
     """dtype = bf16_f32acc (csrc/mlp_tc.cuh): every GEMM-shaped piece of the time loop -- the hidden-layer products of f and
-    of its VJP, and ALL parameter-gradient contractions over the members -- runs on tcgen05 with bf16 operands and fp32 TMEM
+    of its VJP, and ALL parameter-gradient contractions over the members -- runs on wgmma with bf16 operands and fp32 register
     accumulators.  BASELINE C4: <= 2e-2 relative to the fp64 oracle for the bf16 path (observed 1e-3 .. 7e-3)."""
     T, dt = 1.5, 0.05
     saveat = np.linspace(0.05, T, 30)
     rng = np.random.default_rng(0)
     u0 = rng.uniform(-2, 2, (2, N)); p = _weights()
     dL = None if cost == "affine" else rng.standard_normal((30, 2, N))
-    # N = 100, 4096: the 32-member layout (mlp_tc.cuh); N = 12000 (> 2 x 148 x 32): the 128-member layout (mlp_tc_wide.cuh)
+    # N = 100, 4096: the 32-member layout (mlp_tc.cuh); N = 12000 (> 2 x 132 x 32): the 128-member layout (mlp_tc_wide.cuh)
     cfg = O.make_cfg("mlp", sensealg, "tsit5_fixed", N, saveat, 0.0, T, dt=dt, cost=("affine", 1.0, -0.5) if cost == "affine" else ("explicit",), mlp_hidden=H)
     ref = O.gradient(cfg, saveat, u0, p, dLdu=dL)
     eng = b.DeviceEnsemble("mlp", sensealg, "tsit5_fixed", N, saveat, (0.0, T), dt, dtype="bf16_f32acc",
