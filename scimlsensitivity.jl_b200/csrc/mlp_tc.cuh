@@ -170,8 +170,10 @@ __device__ __forceinline__ void tc_setup(TcSmem& s, const float* p) {
     __syncthreads();
 }
 
+// the previous stage's gradient GEMMs read ALL rows of the tiles, and wgmma.wait_group only covers the executing thread's
+// part of them: every warp's wait must have returned (the barrier) before any thread overwrites a tile row
 __device__ __forceinline__ void tc_wait_grad(TcState& st) {
-    if (st.gpend) { wgmma_wait_all(); st.gpend = false; }
+    if (st.gpend) { wgmma_wait_all(); __syncthreads(); st.gpend = false; }
 }
 
 // F = f(y) for this thread's member; leaves H1 (bf16) in TB and this thread's H2 quarter in registers
@@ -314,7 +316,7 @@ __global__ void __launch_bounds__(TC_M) mlp_tc_forward_kernel(const __grid_const
             tc_forward<false>(s, st, y[0], y[1], F, H2q);
             if (sg < 6) { kf[sg][0] = F[0]; kf[sg][1] = F[1]; }
         }
-        if (writer && a.kst) {
+        if (writer) {
             // the dense forward solution of this step (k1..k6, k7 = f(u_{n+1})): the reverse pass reads it back instead of
             // repeating the six stage evaluations (6 of its 18 tensor-core round trips per step), 56 B per member-step
             float* ks_ = a.kst + ((int64_t)n * 14) * N + col;
@@ -354,27 +356,13 @@ __global__ void __launch_bounds__(TC_M) mlp_tc_reverse_kernel(const __grid_const
     };
     uhi[0] = a.ckpt[((int64_t)a.S * 2) * N + col]; uhi[1] = a.ckpt[((int64_t)a.S * 2 + 1) * N + col];
     { const int ks = a.save_of_step[a.S]; if (ks >= 0) cotangent(ks, uhi); }
-    if (!a.kst) tc_forward<true>(s, st, uhi[0], uhi[1], kf[6], H2q);    // f(u_S) = forward k7 of the last step
     for (int n = a.S - 1; n >= 0; n--) {
         ulo[0] = a.ckpt[((int64_t)n * 2) * N + col]; ulo[1] = a.ckpt[((int64_t)n * 2 + 1) * N + col];
-        // ---- forward stages k1..k7 of [t_n, t_{n+1}]: read back from the forward pass (a.kst) or recomputed ----
-        if (a.kst) {
+        // ---- forward stages k1..k7 of [t_n, t_{n+1}]: read back from the forward pass ----
+        {
             const float* ks_ = a.kst + ((int64_t)n * 14) * N + col;
 #pragma unroll
             for (int j = 0; j < 7; j++) { kf[j][0] = ks_[(int64_t)(2 * j) * N]; kf[j][1] = ks_[(int64_t)(2 * j + 1) * N]; }
-        } else {
-            tc_forward<true>(s, st, ulo[0], ulo[1], kf[0], H2q);
-#pragma unroll 1
-            for (int sg = 1; sg <= 5; sg++) {
-                float y[2];
-#pragma unroll
-                for (int c = 0; c < 2; c++) {
-                    double acc = (double)ulo[c];
-                    for (int j = 0; j < sg; j++) acc = fma(tb.hA[sg][j], (double)kf[j][c], acc);
-                    y[c] = (float)acc;
-                }
-                tc_forward<true>(s, st, y[0], y[1], kf[sg], H2q);
-            }
         }
         // ---- adjoint stages 0..5 (GaussAdjoint: 0..6, the 7th derivative feeds the dense output of the adjoint step) ----
 #pragma unroll 1
@@ -418,7 +406,6 @@ __global__ void __launch_bounds__(TC_M) mlp_tc_reverse_kernel(const __grid_const
         }
         { const int ks = a.save_of_step[n]; if (ks >= 0 && !((a.flags & 1u) && n == 0)) cotangent(ks, ulo); }
         uhi[0] = ulo[0]; uhi[1] = ulo[1];
-        if (!a.kst) { kf[6][0] = kf[0][0]; kf[6][1] = kf[0][1]; }
     }
     if (writer) { a.du0[col] = lam[0]; a.du0[N + col] = lam[1]; }
     // ---- parameter gradient of this CTA out of the accumulator fragments ----

@@ -57,19 +57,18 @@ BLOCKS = {"W1": slice(0, 2 * H), "b1": slice(2 * H, 3 * H), "W2": slice(3 * H, 3
           "W3": slice(4 * H + H * H, 6 * H + H * H), "b3": slice(6 * H + H * H, P)}
 
 
-@pytest.mark.parametrize("N", [100, 4096, 12000])
-@pytest.mark.parametrize("cost", ["affine", "explicit"])
-@pytest.mark.parametrize("sensealg", ["interpolating", "gauss"])
-def test_mlp_bf16_tensor_core_path(N, cost, sensealg):
-    """dtype = bf16_f32acc (csrc/mlp_tc.cuh): every GEMM-shaped piece of the time loop -- the hidden-layer products of f and
-    of its VJP, and ALL parameter-gradient contractions over the members -- runs on wgmma with bf16 operands and fp32 register
-    accumulators.  BASELINE C4: <= 2e-2 relative to the fp64 oracle for the bf16 path (observed 1e-3 .. 7e-3)."""
+def _nsm():
+    import torch
+    return torch.cuda.get_device_properties(0).multi_processor_count
+
+
+def _bf16_vs_oracle(N, cost, sensealg, seed=0):
+    """dtype = bf16_f32acc against the fp64 oracle at BASELINE C4's bounds, plus same-launch determinism; -> (dp, oracle dp)"""
     T, dt = 1.5, 0.05
     saveat = np.linspace(0.05, T, 30)
-    rng = np.random.default_rng(0)
+    rng = np.random.default_rng(seed)
     u0 = rng.uniform(-2, 2, (2, N)); p = _weights()
     dL = None if cost == "affine" else rng.standard_normal((30, 2, N))
-    # N = 100, 4096: the 32-member layout (mlp_tc.cuh); N = 12000 (> 2 x 132 x 32): the 128-member layout (mlp_tc_wide.cuh)
     cfg = O.make_cfg("mlp", sensealg, "tsit5_fixed", N, saveat, 0.0, T, dt=dt, cost=("affine", 1.0, -0.5) if cost == "affine" else ("explicit",), mlp_hidden=H)
     ref = O.gradient(cfg, saveat, u0, p, dLdu=dL)
     eng = b.DeviceEnsemble("mlp", sensealg, "tsit5_fixed", N, saveat, (0.0, T), dt, dtype="bf16_f32acc",
@@ -81,17 +80,73 @@ def test_mlp_bf16_tensor_core_path(N, cost, sensealg):
     assert _rel(du0, ref["du0"]) < 1e-2
     for name, sl in BLOCKS.items():
         assert _rel(np.asarray(dp)[sl], ref["dp"][sl]) < 2e-2, name
-    err = np.abs(np.asarray(dp)[BLOCKS["W2"]] - ref["dp"][BLOCKS["W2"]]) / np.abs(ref["dp"][BLOCKS["W2"]]).max()
-    assert np.sqrt(np.mean(err ** 2)) < 2e-3                           # typical error: bf16 rounding averaged over the contraction
     # deterministic: same launch, same bits
     du0b, dpb = eng.reverse(dL)
     assert np.array_equal(np.asarray(du0), np.asarray(du0b)) and np.array_equal(np.asarray(dp), np.asarray(dpb))
     eng.close()
+    return np.asarray(dp), ref["dp"]
+
+
+@pytest.mark.parametrize("N", [100, 4096, 12000])
+@pytest.mark.parametrize("cost", ["affine", "explicit"])
+@pytest.mark.parametrize("sensealg", ["interpolating", "gauss"])
+def test_mlp_bf16_tensor_core_path(N, cost, sensealg):
+    """dtype = bf16_f32acc (csrc/mlp_tc.cuh): every GEMM-shaped piece of the time loop -- the hidden-layer products of f and
+    of its VJP, and ALL parameter-gradient contractions over the members -- runs on wgmma with bf16 operands and fp32 register
+    accumulators.  BASELINE C4: <= 2e-2 relative to the fp64 oracle for the bf16 path (observed 1e-3 .. 7e-3)."""
+    # N = 100, 4096: the 32-member layout (mlp_tc.cuh); N = 12000 (> 64 x 132 SMs): the 128-member layout (mlp_tc_wide.cuh)
+    dp, ref_dp = _bf16_vs_oracle(N, cost, sensealg)
+    err = np.abs(dp[BLOCKS["W2"]] - ref_dp[BLOCKS["W2"]]) / np.abs(ref_dp[BLOCKS["W2"]]).max()
+    assert np.sqrt(np.mean(err ** 2)) < 2e-3                           # typical error: bf16 rounding averaged over the contraction
+
+
+# The host runs the 32-member layout while ceil(N / 32) <= 2 x n_SM, i.e. up to N = 64 n_SM, and the 128-member layout beyond.
+LAYOUT_SIZES = {"1": lambda nsm: 1, "33": lambda nsm: 33, "last_narrow": lambda nsm: 64 * nsm,
+                "first_wide": lambda nsm: 64 * nsm + 1, "wide_last_tile_127": lambda nsm: 64 * nsm + 127}
+
+
+@pytest.mark.parametrize("size", list(LAYOUT_SIZES))
+@pytest.mark.parametrize("sensealg", ["interpolating", "gauss"])
+def test_mlp_bf16_layout_boundaries(size, sensealg):
+    """Both sides of the narrow -> wide switch, which follows the device's SM count: a single member, one full narrow CTA + 1,
+    the largest narrow size, the first wide size (its last 128-member tile holds ONE live member) and a last tile of 127."""
+    _bf16_vs_oracle(LAYOUT_SIZES[size](_nsm()), "affine", sensealg, seed=5)
+
+
+@pytest.mark.parametrize("layout", ["narrow", "wide"])
+@pytest.mark.parametrize("sensealg", ["interpolating", "gauss"])
+def test_mlp_bf16_member_permutation(layout, sensealg):
+    """A member's trajectory and adjoint depend only on its own MMA row: moving every member to another CTA and another row
+    of it (a cyclic shift) leaves saved and du0 bit-identical; dp, a sum over CTAs in another order, agrees to 1e-5."""
+    nsm = _nsm()
+    N, tile = (64 * nsm - 45, 32) if layout == "narrow" else (64 * nsm + 77, 128)     # both with a ragged last tile
+    shift = 1061                                               # 8 x 128 + 37
+    order = np.roll(np.arange(N), shift)                       # position q runs member order[q]; member m sits at (m + shift) % N
+    pos = (np.arange(N) + shift) % N
+    assert ((pos // tile) != (np.arange(N) // tile)).all() and ((pos % tile) != (np.arange(N) % tile)).all()
+    T, dt = 1.5, 0.05
+    saveat = np.linspace(0.05, T, 30)
+    rng = np.random.default_rng(6)
+    u0 = rng.uniform(-2, 2, (2, N)); p = _weights()
+    out = []
+    for perm in (np.arange(N), order):
+        eng = b.DeviceEnsemble("mlp", sensealg, "tsit5_fixed", N, saveat, (0.0, T), dt, dtype="bf16_f32acc", cost=b.AffineCost(1.0, -0.5))
+        saved, _ = eng.forward(u0[:, perm], p)
+        du0, dp = eng.reverse()
+        saved, du0 = np.array(saved), np.array(du0)
+        saved[..., perm] = saved.copy(); du0[:, perm] = du0.copy()                # back to member order
+        out.append((saved, du0, np.array(dp)))
+        eng.close()
+    (s0, u0_, p0), (s1, u1, p1) = out
+    assert np.array_equal(s0, s1)
+    assert np.array_equal(u0_, u1)
+    assert _rel(p1, p0) < 1e-5
 
 
 def test_mlp_bf16_members_not_a_multiple_of_the_tile():
-    """N = 130 = one full 128-member tile + 2: the pad rows of the second tile must contribute nothing to any gradient."""
-    N, T, dt = 130, 1.5, 0.05
+    """N = 64 n_SM + 2, among the first sizes of the 128-member layout: the last tile holds 2 live members and 126 pad rows,
+    which must contribute nothing to any gradient."""
+    N, T, dt = 64 * _nsm() + 2, 1.5, 0.05
     saveat = np.linspace(0.05, T, 30)
     rng = np.random.default_rng(3)
     u0 = rng.uniform(-2, 2, (2, N)); p = _weights()
