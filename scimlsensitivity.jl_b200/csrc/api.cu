@@ -60,9 +60,7 @@ void tsit5_weights(double th, double* w, double (*Rout)[4]) {
     if (Rout) for (int j = 0; j < 7; j++) for (int m = 0; m < 4; m++) Rout[j][m] = R[j][m + 1];
     if (w) for (int j = 0; j < 7; j++) w[j] = (((R[j][4] * th + R[j][3]) * th + R[j][2]) * th + R[j][1]) * th + R[j][0];
 }
-}  // namespace b200adj
 
-namespace {
 // Step-size-scaled Tsit5 tables for one handle (passed to the kernels by value, i.e. through the constant bank).
 void build_tsit5_tables(double h, Tsit5Tables* t) {
     const double A[7][6] = {
@@ -82,7 +80,22 @@ void build_tsit5_tables(double h, Tsit5Tables* t) {
     const double thq[3] = {0.5 * (1.0 - a), 0.5, 0.5 * (1.0 + a)};
     for (int g = 0; g < 3; g++) { tsit5_weights(thq[g], w); for (int j = 0; j < 7; j++) t->hBq[g][j] = h * w[j]; }
     t->hGW[0] = 0.5 * h * (5.0 / 9.0); t->hGW[1] = 0.5 * h * (8.0 / 9.0); t->hGW[2] = 0.5 * h * (5.0 / 9.0);
+    // Hermite form (ode_tsit5.cuh, tsit5_dense_hermite): the 4 stage times of hBst, then the y-side Gauss nodes hBq[2 - g]
+    const double thh[7] = {1.0 - C[1], 1.0 - C[2], 1.0 - C[3], 1.0 - C[4], thq[2], thq[1], thq[0]};
+    for (int r = 0; r < 7; r++) {
+        const double x = thh[r], x2 = x * x, x3 = x2 * x;
+        t->hHm[r][0] = 3.0 * x2 - 2.0 * x3;
+        t->hHm[r][1] = h * (x - 2.0 * x2 + x3);
+        t->hHm[r][2] = h * (x3 - x2);
+        t->hHm[r][3] = x2 * (1.0 - x) * (1.0 - x);
+    }
+    double R[7][4];
+    tsit5_weights(0.0, nullptr, R);
+    for (int j = 0; j < 7; j++) t->hR4[j] = h * R[j][3];
 }
+}  // namespace b200adj
+
+namespace {
 T5aArgs t5a_args(Handle* h) {
     const b200adj_cfg& c = h->cfg;
     T5aArgs a;

@@ -105,11 +105,14 @@ inline bool is_sde(const b200adj_cfg& c) { return c.stepper == B200ADJ_ST_EM || 
 inline size_t esz(const b200adj_cfg& c) { return c.dtype == B200ADJ_F64 ? sizeof(double) : sizeof(float); }   // BF16_F32ACC: fp32 buffers at the ABI
 
 void tsit5_weights(double th, double* w, double (*Rout)[4] = nullptr);
+void build_tsit5_tables(double h, Tsit5Tables* t);
 template <class T, class S> inline void cast_tables(const S& src, T* dst) {
     for (int i = 0; i < 7; i++) for (int j = 0; j < 6; j++) dst->hA[i][j] = (float)src.hA[i][j];
     for (int i = 0; i < 4; i++) for (int j = 0; j < 7; j++) dst->hBst[i][j] = (float)src.hBst[i][j];
     for (int i = 0; i < 3; i++) for (int j = 0; j < 7; j++) dst->hBq[i][j] = (float)src.hBq[i][j];
     for (int i = 0; i < 3; i++) dst->hGW[i] = (float)src.hGW[i];
+    for (int i = 0; i < 7; i++) for (int j = 0; j < 4; j++) dst->hHm[i][j] = (float)src.hHm[i][j];
+    for (int j = 0; j < 7; j++) dst->hR4[j] = (float)src.hR4[j];
 }
 
 

@@ -34,6 +34,11 @@ template <class R> struct Tsit5TablesT {
     R hBst[4][7];  // h * b_j(theta) at theta = 1 - c_s for adjoint stages s = 1..4 (0-based)
     R hBq[3][7];   // h * b_j(theta) at theta = (1 -/+ sqrt(.6))/2, 1/2  (3-pt Gauss-Legendre nodes)
     R hGW[3];      // (h/2) * Gauss-Legendre weights 5/9, 8/9, 5/9
+    // Hermite form of the forward dense output (tsit5_dense_hermite): per point {H01, h*H10, h*H11, theta^2 (1-theta)^2}
+    // at the 4 adjoint stage times (rows 0..3, theta of hBst) and at the y-side Gauss nodes (rows 4..6: row 4 + g has the
+    // theta of hBq[2 - g]), and hR4 = h * (theta^4 coefficient of b_j)
+    R hHm[7][4];
+    R hR4[7];
 };
 using Tsit5Tables = Tsit5TablesT<double>;
 
@@ -149,6 +154,25 @@ template <int D, class R> __device__ __forceinline__ void tsit5_dense(const R* u
         for (int j = 0; j < 7; j++) acc = fma(w[j], k[j][i], acc);
         out[i] = acc;
     }
+}
+// The same dense output in Hermite form.  The Tsit5 interpolant is a C1 Hermite quartic: b_j(1) = b_j (row 6 of hA / h),
+// b_j'(0) = delta_j1, b_j'(1) = delta_j7, so with du = u_{n+1} - u_n, k1, k7 = f(u_{n+1}) and c4 = sum_j hR4[j] k_j
+//   y(theta) = u_n + H01 du + h H10 k1 + h H11 k7 + theta^2 (1-theta)^2 c4
+// (H01 = 3t^2 - 2t^3, H10 = t - 2t^2 + t^3, H11 = t^3 - t^2): 4 FMAs per component once c4 and du are formed, against
+// 7 for tsit5_dense.  All weights are <= 1 in magnitude.  u_{n+1} and k7 must be the end point of the SAME step as k1..k6.
+template <int D, class R> __device__ __forceinline__ void tsit5_hermite_c4(const Tsit5TablesT<R>& tb, const R (*k)[D], R* c4) {
+#pragma unroll
+    for (int i = 0; i < D; i++) {
+        R acc = tb.hR4[0] * k[0][i];
+#pragma unroll
+        for (int j = 1; j < 7; j++) acc = fma(tb.hR4[j], k[j][i], acc);
+        c4[i] = acc;
+    }
+}
+template <int D, class R>
+__device__ __forceinline__ void tsit5_dense_hermite(const R* u, const R* du, const R* k1, const R* k7, const R* c4, const R* w, R* out) {
+#pragma unroll
+    for (int i = 0; i < D; i++) out[i] = fma(w[3], c4[i], fma(w[2], k7[i], fma(w[1], k1[i], fma(w[0], du[i], u[i]))));
 }
 
 // producer/consumer named barriers (ids 1..15; id 0 is __syncthreads)
@@ -467,7 +491,7 @@ __global__ void __maxnreg__(B200_REV_MAXREG) tsit5_reverse_kernel(const __grid_c
     } else {
         R kf[7][D];                       // forward stages of the current step; kf[6] = f(u_{n+1}) carried over
         R ka[7][D];                       // adjoint stages (+J'lam); ka[0] carried over (FSAL) unless a jump hit
-        R ulo[D], uhi[D];                 // uhi (= u_{n+1}) is live only for SA_INTERP
+        R ulo[D], uhi[D];                 // u_n, u_{n+1} (the end point of the Hermite dense output)
         // Forward checkpoints are staged HBM -> shared memory by TMA bulk copies, CH steps per stage, NST stages in
         // flight, completion tracked by one mbarrier per stage.  A register prefetch does not survive the register
         // cap (ptxas sinks the LDG next to its use and every step then eats a full DRAM latency -- 32% of all
@@ -605,6 +629,12 @@ __global__ void __maxnreg__(B200_REV_MAXREG) tsit5_reverse_kernel(const __grid_c
                 add_continuous<D, CONT>(a, uhi, ka[0]);
                 need_left = false;
             }
+            // Hermite data of the forward dense output: uhi / kf[6] are this step's end point (the checkpoint u_{n+1} and its
+            // FSAL derivative, or the re-derived left limit at an event); kf[1..5] are dead from here on (except for GK)
+            R du[D], c4[D];
+            tsit5_hermite_c4<D>(tb, kf, c4);
+#pragma unroll
+            for (int j = 0; j < D; j++) du[j] = uhi[j] - ulo[j];
 #ifdef REV_MIDSYNC
             __syncthreads();
 #endif
@@ -622,10 +652,10 @@ __global__ void __maxnreg__(B200_REV_MAXREG) tsit5_reverse_kernel(const __grid_c
             Fam::vjp_u(y, p, ls, ka[S_]); add_continuous<D, CONT>(a, y, ka[S_]);                 \
             if (SA == SA_INTERP && S_ < 6) { Fam::vjp_p(y, p, ls, dg);                     \
                 _Pragma("unroll") for (int q = 0; q < P; q++) mu[q] = fma(tb.hA[6][S_ < 6 ? S_ : 0], dg[q], mu[q]); }
-            B200_ADJ_STAGE(1, tsit5_dense<D>(ulo, kf, tb.hBst[0], y))
-            B200_ADJ_STAGE(2, tsit5_dense<D>(ulo, kf, tb.hBst[1], y))
-            B200_ADJ_STAGE(3, tsit5_dense<D>(ulo, kf, tb.hBst[2], y))
-            B200_ADJ_STAGE(4, tsit5_dense<D>(ulo, kf, tb.hBst[3], y))
+            B200_ADJ_STAGE(1, tsit5_dense_hermite<D>(ulo, du, kf[0], kf[6], c4, tb.hHm[0], y))
+            B200_ADJ_STAGE(2, tsit5_dense_hermite<D>(ulo, du, kf[0], kf[6], c4, tb.hHm[1], y))
+            B200_ADJ_STAGE(3, tsit5_dense_hermite<D>(ulo, du, kf[0], kf[6], c4, tb.hHm[2], y))
+            B200_ADJ_STAGE(4, tsit5_dense_hermite<D>(ulo, du, kf[0], kf[6], c4, tb.hHm[3], y))
             B200_ADJ_STAGE(5, _Pragma("unroll") for (int j = 0; j < D; j++) y[j] = ulo[j])
             B200_ADJ_STAGE(6, _Pragma("unroll") for (int j = 0; j < D; j++) y[j] = ulo[j])
 #undef B200_ADJ_STAGE
@@ -677,7 +707,7 @@ __global__ void __maxnreg__(B200_REV_MAXREG) tsit5_reverse_kernel(const __grid_c
 #pragma unroll
                 for (int g = 0; g < 3; g++) {
                     tsit5_dense<D>(lam, ka, tb.hBq[g], lq);
-                    tsit5_dense<D>(ulo, kf, tb.hBq[2 - g], y);
+                    tsit5_dense_hermite<D>(ulo, du, kf[0], kf[6], c4, tb.hHm[4 + g], y);
                     Fam::vjp_p(y, p, lq, dg);
 #pragma unroll
                     for (int q = 0; q < P; q++) mu[q] = fma(tb.hGW[g], dg[q], mu[q]);
