@@ -10,22 +10,112 @@ namespace {
 
 thread_local std::string g_create_error;
 
+// Tsit5 tableau (Tsitouras 2011): stage matrix (row 6 = b), nodes, embedded error weights b - bhat
+const double TSIT5_A[7][6] = {
+    {0},
+    {0.161},
+    {-0.008480655492356989, 0.335480655492357},
+    {2.8971530571054935, -6.359448489975075, 4.3622954328695815},
+    {5.325864828439257, -11.748883564062828, 7.4955393428898365, -0.09249506636175525},
+    {5.86145544294642, -12.92096931784711, 8.159367898576159, -0.071584973281401, -0.028269050394068383},
+    {0.09646076681806523, 0.01, 0.4798896504144996, 1.379008574103742, -3.290069515436081, 2.324710524099774}};
+const double TSIT5_C[7] = {0.0, 0.161, 0.327, 0.9, 0.9800255409045097, 1.0, 1.0};
+const double TSIT5_BT[7] = {-0.00178001105222577714, -0.0008164344596567469, 0.007880878010261995, -0.1447110071732629,
+                            0.5823571654525552, -0.45808210592918697, 0.015151515151515152};
+
 // registered plug-in families (append-only; a registration is as global as the dlopen behind it)
 std::vector<const FamilyVTable*>& family_registry() { static std::vector<const FamilyVTable*> r; return r; }
 
+// a built-in ODE family: the launchers its disp_<stepper>_<family>.cu files instantiate
+template <class F, bool FIXED_GRID, bool ROS, bool F32>
+FamilyVTable builtin_family(const char* name) {
+    FamilyVTable v = {B200ADJ_PLUGIN_ABI, F::D, F::P, name};
+    v.t5a_fwd = &launch_t5a_fwd<F>; v.t5a_rev = &launch_t5a_rev<F>;
+    if constexpr (FIXED_GRID) { v.fwd = &launch_fwd<F>; v.rev = &launch_rev<F>; }
+    if constexpr (ROS) { v.ros_fwd = &launch_ros_fwd<F>; v.ros_rev = &launch_ros_rev<F>; }
+    if constexpr (F32) { v.fwd_f32 = &launch_fwd_f32<F>; v.rev_f32 = &launch_rev_f32<F>; }
+    return v;
+}
+constexpr int BUILTIN_FAMILIES = B200ADJ_FAM_RELAX + 1;
+const FamilyVTable* builtin_families() {        // indexed by B200ADJ_FAM_*; abi == 0: an SDE / MLP family (own dispatch)
+    static const FamilyVTable t[BUILTIN_FAMILIES] = {
+        builtin_family<LotkaVolterra, true, true, true>("lv"),
+        builtin_family<Lorenz, true, true, true>("lorenz"),
+        builtin_family<Robertson, true, true, false>("robertson"),
+        {}, {}, {},                             // SDE_LV, MLP, SDE_LINEAR
+        builtin_family<BouncingBall, false, false, false>("ball"),
+        builtin_family<Relax, false, false, false>("relax")};
+    return t;
+}
+
+// d, P, m of the families with their own dispatch entry points (sde_*_dispatch, mlp_*_dispatch)
+struct FamDims { int32_t id, d, P, m; };
+constexpr FamDims OWN_DISPATCH_FAMILIES[] = {
+    {B200ADJ_FAM_SDE_LV, SdeLotkaVolterra<false>::D, SdeLotkaVolterra<false>::P, SdeLotkaVolterra<false>::M},
+    {B200ADJ_FAM_SDE_LINEAR, SdeLinear2<false>::D, SdeLinear2<false>::P, SdeLinear2<false>::M},
+    {B200ADJ_FAM_MLP, MLP_D, MLP_P, 0}};
+
 int fam_dims(const b200adj_cfg& c, int* d, int* P, int* m) {
     if (const FamilyVTable* vt = family_lookup(c.rhs_family)) { *d = vt->d; *P = vt->P; *m = 0; return 0; }
-    switch (c.rhs_family) {
-    case B200ADJ_FAM_LV: *d = 2; *P = 4; *m = 0; return 0;
-    case B200ADJ_FAM_LORENZ: *d = 3; *P = 3; *m = 0; return 0;
-    case B200ADJ_FAM_ROBERTSON: *d = 3; *P = 3; *m = 0; return 0;
-    case B200ADJ_FAM_SDE_LV: *d = 2; *P = 6; *m = 2; return 0;
-    case B200ADJ_FAM_SDE_LINEAR: *d = 2; *P = 2; *m = 2; return 0;
-    case B200ADJ_FAM_BALL: *d = 2; *P = 2; *m = 0; return 0;
-    case B200ADJ_FAM_RELAX: *d = 1; *P = 2; *m = 0; return 0;
-    case B200ADJ_FAM_MLP: if (c.mlp_hidden != MLP_H) return -1; *d = MLP_D; *P = MLP_P; *m = 0; return 0;
-    default: return -1;
+    if (c.rhs_family == B200ADJ_FAM_MLP && c.mlp_hidden != MLP_H) return -1;
+    for (const FamDims& f : OWN_DISPATCH_FAMILIES)
+        if (f.id == c.rhs_family) { *d = f.d; *P = f.P; *m = f.m; return 0; }
+    return -1;
+}
+
+// The support matrix: is `sensealg` built for this execution path, dtype and checkpointing, with preset-time events and a
+// continuous callback on the handle or not?  B200ADJ_ERR_UNSUPPORTED with the refused feature in `err`, INVALID for an
+// unknown ODE sensealg.  The rules come in groups (`rules`) so that b200adj_create can ask each group at the point of its
+// validation sequence where that group decides the returned code; the setters ask all of them.
+enum SupportRules : unsigned {
+    SR_DTYPE = 1,          // QuadratureAdjoint is F64 only
+    SR_MLP = 2,            // MLP family: Interpolating / Gauss
+    SR_SENSEALG = 4,       // SDE: Backsolve / Interpolating; known sensealg; GaussKronrod F64 only
+    SR_CKPT = 8,           // checkpoint_every > 1: fixed-step Tsit5 with Interpolating / Gauss
+    SR_CALLBACKS = 16,     // QuadratureAdjoint: no events, no continuous callback
+    SR_ALL = 31
+};
+int32_t check_support(const b200adj_cfg& c, Path path, int ckpt_every, int32_t sensealg, bool events, bool callback, std::string& err,
+                      unsigned rules = SR_ALL) {
+    auto refuse = [&](const char* msg) { err = msg; return B200ADJ_ERR_UNSUPPORTED; };
+    const bool interp_gauss = sensealg == B200ADJ_SA_INTERPOLATING || sensealg == B200ADJ_SA_GAUSS;
+    if ((rules & SR_DTYPE) && sensealg == B200ADJ_SA_QUADRATURE && c.dtype != B200ADJ_F64) return refuse("F32: QuadratureAdjoint is F64 only");
+    if ((rules & SR_MLP) && path == Path::MLP && !interp_gauss) return refuse("MLP family: InterpolatingAdjoint / GaussAdjoint are built");
+    if (rules & SR_SENSEALG) {
+        if (path == Path::SDE && sensealg != B200ADJ_SA_BACKSOLVE && sensealg != B200ADJ_SA_INTERPOLATING)
+            return refuse("SDE: BacksolveAdjoint / InterpolatingAdjoint are built");
+        if (sensealg < 0 || sensealg > 4) { err = "bad sensealg"; return B200ADJ_ERR_INVALID; }
+        if (sensealg == B200ADJ_SA_GAUSSKRONROD && c.dtype != B200ADJ_F64) return refuse("GaussKronrodAdjoint: F64, named ODE families");
     }
+    if ((rules & SR_CKPT) && ckpt_every > 1 && (path == Path::MLP || path == Path::SDE || !interp_gauss))
+        return refuse("checkpoint_every > 1: fixed-step Tsit5 with InterpolatingAdjoint / GaussAdjoint (the sensealgs that checkpoint in the reference)");
+    if ((rules & SR_CALLBACKS) && sensealg == B200ADJ_SA_QUADRATURE && events) return refuse("events: QuadratureAdjoint has no callback support");
+    if ((rules & SR_CALLBACKS) && sensealg == B200ADJ_SA_QUADRATURE && callback) return refuse("continuous callback: QuadratureAdjoint has no callback support");
+    return B200ADJ_OK;
+}
+int32_t check_support(Handle* h, int32_t sensealg, bool events, bool callback) {
+    return check_support(h->cfg, h->path, h->ckpt_every, sensealg, events, callback, h->err);
+}
+
+// a device copy of a host table, at least one element long so that the pointer is valid for an empty table
+template <class T> cudaError_t upload_table(T** dst, const T* src, size_t n) {
+    cudaError_t e = cudaMalloc(dst, (n > 0 ? n : 1) * sizeof(T));
+    if (e == cudaSuccess && n > 0) e = cudaMemcpy(*dst, src, n * sizeof(T), cudaMemcpyHostToDevice);
+    return e;
+}
+
+// staging buffers of forward / reverse for host pointers (buffers_on_device == 0)
+cudaError_t alloc_staging(Handle* h) {
+    const b200adj_cfg& c = h->cfg;
+    const size_t N = (size_t)c.N, e = esz(c), dn = (size_t)c.d * N, pn = c.shared_p ? (size_t)c.P : (size_t)c.P * N;
+    cudaError_t r = cudaSuccess;
+    auto get = [&](auto** p, size_t bytes) { if (r == cudaSuccess) r = cudaMalloc(p, bytes); };
+    get(&h->s_u0, dn * e); get(&h->s_p, pn * e); get(&h->s_du0, dn * e); get(&h->s_dp, pn * e); get(&h->s_status, N * sizeof(int32_t));
+    if (c.K > 0) {
+        get(&h->s_saved, (size_t)c.K * dn * e);
+        if (c.cost_kind == B200ADJ_COST_EXPLICIT) get(&h->s_dLdu, (size_t)c.K * dn * e);
+    }
+    return r;
 }
 }  // namespace
 
@@ -63,15 +153,8 @@ void tsit5_weights(double th, double* w, double (*Rout)[4]) {
 
 // Step-size-scaled Tsit5 tables for one handle (passed to the kernels by value, i.e. through the constant bank).
 void build_tsit5_tables(double h, Tsit5Tables* t) {
-    const double A[7][6] = {
-        {0},
-        {0.161},
-        {-0.008480655492356989, 0.335480655492357},
-        {2.8971530571054935, -6.359448489975075, 4.3622954328695815},
-        {5.325864828439257, -11.748883564062828, 7.4955393428898365, -0.09249506636175525},
-        {5.86145544294642, -12.92096931784711, 8.159367898576159, -0.071584973281401, -0.028269050394068383},
-        {0.09646076681806523, 0.01, 0.4798896504144996, 1.379008574103742, -3.290069515436081, 2.324710524099774}};
-    const double C[7] = {0.0, 0.161, 0.327, 0.9, 0.9800255409045097, 1.0, 1.0};
+    const double (&A)[7][6] = TSIT5_A;
+    const double (&C)[7] = TSIT5_C;
     memset(t, 0, sizeof(*t));
     for (int s = 0; s < 7; s++) for (int j = 0; j < 6; j++) t->hA[s][j] = h * A[s][j];
     double w[7];
@@ -93,37 +176,62 @@ void build_tsit5_tables(double h, Tsit5Tables* t) {
     tsit5_weights(0.0, nullptr, R);
     for (int j = 0; j < 7; j++) t->hR4[j] = h * R[j][3];
 }
+
+const FamilyVTable* family_lookup(int id) {
+    if (id >= 0 && id < BUILTIN_FAMILIES) { const FamilyVTable* vt = &builtin_families()[id]; return vt->abi ? vt : nullptr; }
+    auto& r = family_registry();
+    const int k = id - B200ADJ_FAM_USER_BASE_ID;
+    return (k >= 0 && k < (int)r.size()) ? r[k] : nullptr;
+}
+
+// QuadratureAdjoint's buffers, allocated at its first reverse pass (no other sensealg needs them): the dense reverse solution
+// (FIXED: [S][8][d][Npad]; T5A / ROS: member-major records), on ROS the member-major copy of the forward one (T5A keeps
+// the forward solution member-major from the start), and the quadgk scratch
+int ensure_quad_buffers(Handle* h) {
+    const b200adj_cfg& c = h->cfg;
+    const size_t N = (size_t)c.N, MS = (size_t)h->maxs;
+    auto get = [](double** p, size_t n) { return *p || cudaMalloc(p, n * sizeof(double)) == cudaSuccess; };
+    bool ok;
+    if (h->path == Path::FIXED) {
+        ok = get(&h->d_adj_dense, (size_t)h->S * 8 * c.d * (size_t)h->Npad);
+    } else {
+        const int nk = h->path == Path::ROS ? 2 : 7;      // dense-output stages stored per step
+        const size_t RWP = quad_pad(3 + (1 + nk) * c.d), FWP = quad_pad((1 + nk) * c.d + 3);
+        ok = get(&h->r_rrec, N * MS * RWP) && get(&h->r_rend, N * MS) &&
+             (h->path == Path::T5A || (get(&h->r_ftT, N * (MS + 1)) && get(&h->r_frecT, N * MS * FWP)));
+    }
+    ok = ok && get(&h->r_qseg, quad_seg_doubles(c.P, h->maxseg, h->qgrid)) && get(&h->r_qkey, (size_t)h->qgrid * QUAD_WARPS * h->maxseg);
+    if (!ok) {
+        cudaGetLastError();
+        h->err = "out of device memory for the QuadratureAdjoint buffers (dense reverse solution and quadgk scratch)";
+        return B200ADJ_ERR_OOM;
+    }
+    return B200ADJ_OK;
+}
 }  // namespace b200adj
 
 namespace {
-T5aArgs t5a_args(Handle* h) {
+// the fields T5aArgs and RosArgs share
+template <class A> A dense_args(Handle* h) {
     const b200adj_cfg& c = h->cfg;
-    T5aArgs a;
+    A a;
     memset(&a, 0, sizeof(a));
     a.saveat = h->d_saveat; a.partials = h->d_partials; a.ticket = h->d_ticket;
     a.ft = h->r_ft; a.fu = h->r_fu; a.fk = h->r_fk; a.fn = h->r_fn;
     a.rrec = h->r_rrec; a.rend = h->r_rend; a.ftT = h->r_ftT; a.frecT = h->r_frecT; a.rn = h->r_rn;
     a.qseg = h->r_qseg; a.qkey = h->r_qkey; a.maxseg = h->maxseg;
-    a.N = c.N; a.K = c.K; a.maxs = h->maxs; a.t0 = c.t0; a.t1 = c.t1; a.dt0 = c.dt; a.abstol = c.abstol; a.reltol = c.reltol;
+    a.N = c.N; a.K = c.K; a.maxs = h->maxs; a.t0 = c.t0; a.t1 = c.t1; a.abstol = c.abstol; a.reltol = c.reltol;
     a.quad_abstol = c.quad_abstol; a.quad_reltol = c.quad_reltol;
     for (int j = 0; j < 4; j++) { a.cost_a[j] = h->cost_av[j]; a.cost_b[j] = h->cost_bv[j]; }
-    a.flags = ((c.flags & B200ADJ_FLAG_NO_START) ? 1u : 0u) | ((c.flags & B200ADJ_FLAG_NO_CHECKPOINTING) ? 2u : 0u) |
-              ((c.flags & B200ADJ_FLAG_CKPT_EVERY_STEP) ? 4u : 0u);
-    const double A[7][6] = {
-        {0},
-        {0.161},
-        {-0.008480655492356989, 0.335480655492357},
-        {2.8971530571054935, -6.359448489975075, 4.3622954328695815},
-        {5.325864828439257, -11.748883564062828, 7.4955393428898365, -0.09249506636175525},
-        {5.86145544294642, -12.92096931784711, 8.159367898576159, -0.071584973281401, -0.028269050394068383},
-        {0.09646076681806523, 0.01, 0.4798896504144996, 1.379008574103742, -3.290069515436081, 2.324710524099774}};
-    const double C[7] = {0.0, 0.161, 0.327, 0.9, 0.9800255409045097, 1.0, 1.0};
-    const double BT[7] = {-0.00178001105222577714, -0.0008164344596567469, 0.007880878010261995, -0.1447110071732629,
-                          0.5823571654525552, -0.45808210592918697, 0.015151515151515152};
-    memcpy(a.A, A, sizeof(A)); memcpy(a.C, C, sizeof(C)); memcpy(a.BT, BT, sizeof(BT));
+    a.flags = kernel_flags(h);
+    return a;
+}
+T5aArgs t5a_args(Handle* h) {
+    T5aArgs a = dense_args<T5aArgs>(h);
+    a.dt0 = h->cfg.dt;
+    memcpy(a.A, TSIT5_A, sizeof(TSIT5_A)); memcpy(a.C, TSIT5_C, sizeof(TSIT5_C)); memcpy(a.BT, TSIT5_BT, sizeof(TSIT5_BT));
     tsit5_weights(0.0, nullptr, a.R);
-    if (h->fixed_dt) a.flags |= 16u;          // constant step, no error control (fixed-step Tsit5 on the dense framework)
-    if (h->cont_on) { a.flags |= 8u; for (int j = 0; j < 4; j++) { a.cont_a[j] = h->cont_av[j]; a.cont_b[j] = h->cont_bv[j]; } }
+    if (h->cont_on) for (int j = 0; j < 4; j++) { a.cont_a[j] = h->cont_av[j]; a.cont_b[j] = h->cont_bv[j]; }
     a.nev = h->nev; a.ev_t = h->d_ev_t; a.ev_s = h->d_ev_s; a.ev_c = h->d_ev_c; a.ev_ps = h->d_ev_ps; a.ev_pc = h->d_ev_pc;
     a.ev_ac = h->d_ev_ac; a.ev_ak = h->d_ev_ak; a.ev_af = h->d_ev_af;
     if (h->cc_on) {
@@ -135,21 +243,9 @@ T5aArgs t5a_args(Handle* h) {
     }
     return a;
 }
-RosArgs ros_args(Handle* h) {
-    const b200adj_cfg& c = h->cfg;
-    RosArgs a;
-    memset(&a, 0, sizeof(a));
-    a.saveat = h->d_saveat; a.partials = h->d_partials; a.ticket = h->d_ticket;
-    a.ft = h->r_ft; a.fu = h->r_fu; a.fk = h->r_fk; a.fn = h->r_fn;
-    a.rrec = h->r_rrec; a.rend = h->r_rend; a.ftT = h->r_ftT; a.frecT = h->r_frecT; a.rn = h->r_rn;
-    a.qseg = h->r_qseg; a.qkey = h->r_qkey; a.maxseg = h->maxseg;
-    a.N = c.N; a.K = c.K; a.maxs = h->maxs; a.t0 = c.t0; a.t1 = c.t1; a.abstol = c.abstol; a.reltol = c.reltol;
-    a.quad_abstol = c.quad_abstol; a.quad_reltol = c.quad_reltol;
-    for (int j = 0; j < 4; j++) { a.cost_a[j] = h->cost_av[j]; a.cost_b[j] = h->cost_bv[j]; }
-    a.flags = ((c.flags & B200ADJ_FLAG_NO_START) ? 1u : 0u) | ((c.flags & B200ADJ_FLAG_NO_CHECKPOINTING) ? 2u : 0u) |
-              ((c.flags & B200ADJ_FLAG_CKPT_EVERY_STEP) ? 4u : 0u);
-    return a;
-}
+// a family launcher, or UNSUPPORTED where the family has none for this stepper / dtype
+template <class A> int launch(int (*fn)(Handle*, const A&), Handle* h, const A& a) { return fn ? fn(h, a) : B200ADJ_ERR_UNSUPPORTED; }
+
 void free_all(Handle* h) {
     cudaSetDevice(h->cfg.device);
     cudaFree(h->r_ft); cudaFree(h->r_fu); cudaFree(h->r_fk); cudaFree(h->r_rrec); cudaFree(h->r_rend); cudaFree(h->r_ftT); cudaFree(h->r_frecT);
@@ -161,9 +257,6 @@ void free_all(Handle* h) {
     if (h->own_stream) cudaStreamDestroy(h->own_stream);
 }
 
-}  // namespace
-
-namespace {
 // dp += coef_c .* p + coef_e per member (shared parameters: N times, once)
 struct DgdpArgs { double c[8], e[8]; const void* p; void* dp; int64_t N; int32_t P, shared_p, f32; };
 __global__ void dgdp_add_kernel(DgdpArgs g) {
@@ -183,35 +276,6 @@ __global__ void dgdp_add_kernel(DgdpArgs g) {
     }
 }
 }  // namespace
-
-namespace b200adj {
-const FamilyVTable* family_lookup(int id) {
-    auto& r = family_registry();
-    const int k = id - B200ADJ_FAM_USER_BASE_ID;
-    return (k >= 0 && k < (int)r.size()) ? r[k] : nullptr;
-}
-}  // namespace b200adj
-
-namespace b200adj {
-// QuadratureAdjoint on an adaptive handle: the dense reverse solution, the member-major copy of the forward one and the
-// quadgk scratch are only needed by this sensealg -- allocate them at its first reverse pass
-int ensure_quad_buffers(Handle* h) {
-    if (h->r_rrec) return B200ADJ_OK;
-    const b200adj_cfg& c = h->cfg;
-    const size_t N = (size_t)c.N, MS = (size_t)h->maxs, e = sizeof(double);
-    const size_t RWP = quad_pad(3 + (1 + h->nk) * c.d), FWP = quad_pad((1 + h->nk) * c.d + 3);
-    const bool t5a = h->nk == 7;      // adaptive Tsit5: the forward dense solution is member-major from the start (allocated at create)
-    if (cudaMalloc(&h->r_rrec, N * MS * RWP * e) != cudaSuccess || cudaMalloc(&h->r_rend, N * MS * e) != cudaSuccess ||
-        (!t5a && (cudaMalloc(&h->r_ftT, N * (MS + 1) * e) != cudaSuccess || cudaMalloc(&h->r_frecT, N * MS * FWP * e) != cudaSuccess)) ||
-        cudaMalloc(&h->r_qseg, quad_seg_doubles(c.P, h->maxseg, h->qgrid) * e) != cudaSuccess ||
-        cudaMalloc(&h->r_qkey, (size_t)h->qgrid * QUAD_WARPS * h->maxseg * e) != cudaSuccess) {
-        cudaGetLastError();
-        h->err = "out of device memory for the QuadratureAdjoint buffers (dense reverse solution: N * max_steps records)";
-        return B200ADJ_ERR_OOM;
-    }
-    return B200ADJ_OK;
-}
-}  // namespace b200adj
 
 extern "C" {
 
@@ -237,7 +301,7 @@ int32_t b200adj_create(const b200adj_cfg* cfg, void** handle) {
     // Fixed-step Tsit5 with save times OFF the dt grid (or B200ADJ_FLAG_DENSE_FORWARD): the reference interpolates the dense
     // forward solution at saveat (src/concrete_solve.jl:752-769) and the jump times become tstops of the fixed-dt reverse
     // solve, whose grid then shifts.  That needs the dense forward solution (k1..k7 per step) and general-theta lookups: the
-    // per-member framework of the adaptive steppers run with a constant step (t5a kernels, T5A_FLAG_FIXED_DT).
+    // per-member framework of the adaptive steppers run with a constant step (T5A kernels, KF_FIXED_DT).
     bool dense_fixed = false;
     if (cfg->stepper == B200ADJ_ST_TSIT5_FIXED && cfg->dtype == B200ADJ_F64 && cfg->rhs_family != B200ADJ_FAM_MLP && cfg->dt > 0) {
         dense_fixed = (cfg->flags & B200ADJ_FLAG_DENSE_FORWARD) != 0;
@@ -251,157 +315,99 @@ int32_t b200adj_create(const b200adj_cfg* cfg, void** handle) {
     const bool ros = cfg->stepper == B200ADJ_ST_ROSENBROCK23 || t5a;      // per-member adaptive framework
     if (cfg->N <= 0 || cfg->K < 0 || (cfg->K > 0 && !cfg->saveat) || (!ros && !(cfg->dt > 0)) || !(cfg->t1 > cfg->t0)) {
         g_create_error = "bad N/K/saveat/dt/tspan"; return B200ADJ_ERR_INVALID; }
-    const bool mlp = cfg->rhs_family == B200ADJ_FAM_MLP;
+    const bool mlp = cfg->rhs_family == B200ADJ_FAM_MLP, sde = is_sde(*cfg);
+    const Path path = mlp ? Path::MLP : t5a ? Path::T5A : ros ? Path::ROS : sde ? Path::SDE : Path::FIXED;
+    // interval checkpointing (a14) exists on the fixed grid: forward states every C steps, segments re-solved by the reverse kernel
+    int ckpt_every = (!ros && cfg->checkpoint_every > 1) ? cfg->checkpoint_every : 1;
+    // the support-matrix groups are asked where each decides the returned code among the other checks
+    auto support = [&](unsigned rules) { return check_support(*cfg, path, ckpt_every, cfg->sensealg, false, false, g_create_error, rules); };
     // F32: the MLP family and the fixed-step Tsit5 ODE path of LV / Lorenz (the fp32 throughput variant, SURVEY.md 8d C2)
     const bool f32_ode = cfg->dtype == B200ADJ_F32 && cfg->stepper == B200ADJ_ST_TSIT5_FIXED &&
                          (cfg->rhs_family == B200ADJ_FAM_LV || cfg->rhs_family == B200ADJ_FAM_LORENZ);
-    if (f32_ode && cfg->sensealg == B200ADJ_SA_QUADRATURE) { g_create_error = "F32: Interpolating / Gauss / Backsolve (QuadratureAdjoint is F64 only)"; return B200ADJ_ERR_UNSUPPORTED; }
+    if (int32_t rc = support(SR_DTYPE)) return rc;
     if (cfg->dtype != B200ADJ_F64 && !f32_ode && !(mlp && (cfg->dtype == B200ADJ_F32 || cfg->dtype == B200ADJ_BF16_F32ACC))) {
         g_create_error = "dtype: F64 (all families), F32 (MLP; LV / Lorenz with fixed-step Tsit5), BF16_F32ACC (MLP) are built"; return B200ADJ_ERR_UNSUPPORTED; }
-    if (mlp && (cfg->stepper != B200ADJ_ST_TSIT5_FIXED || (cfg->sensealg != B200ADJ_SA_INTERPOLATING && cfg->sensealg != B200ADJ_SA_GAUSS) || !cfg->shared_p)) {
-        g_create_error = "MLP family: InterpolatingAdjoint / GaussAdjoint + fixed-step Tsit5 + shared parameters are built"; return B200ADJ_ERR_UNSUPPORTED; }
+    if (mlp && (cfg->stepper != B200ADJ_ST_TSIT5_FIXED || !cfg->shared_p)) {
+        g_create_error = "MLP family: fixed-step Tsit5 + shared parameters are built"; return B200ADJ_ERR_UNSUPPORTED; }
+    if (int32_t rc = support(SR_MLP)) return rc;
     if (cfg->cost_kind != B200ADJ_COST_EXPLICIT && cfg->cost_kind != B200ADJ_COST_AFFINE) { g_create_error = "bad cost_kind"; return B200ADJ_ERR_INVALID; }
-    const bool sde = is_sde(*cfg);
-    if (sde) {
-        if (m == 0) { g_create_error = "SDE stepper needs an SDE family"; return B200ADJ_ERR_INVALID; }
-        if (cfg->sensealg != B200ADJ_SA_BACKSOLVE && cfg->sensealg != B200ADJ_SA_INTERPOLATING) { g_create_error = "SDE: BacksolveAdjoint / InterpolatingAdjoint are built"; return B200ADJ_ERR_UNSUPPORTED; }
-    } else {
-        if (m != 0) { g_create_error = "ODE stepper with an SDE family"; return B200ADJ_ERR_INVALID; }
-        if (cfg->sensealg < 0 || cfg->sensealg > 4) { g_create_error = "bad sensealg"; return B200ADJ_ERR_INVALID; }
-        if (cfg->sensealg == B200ADJ_SA_GAUSSKRONROD && (mlp || cfg->dtype != B200ADJ_F64)) { g_create_error = "GaussKronrodAdjoint: F64, named ODE families"; return B200ADJ_ERR_UNSUPPORTED; }
-        if (cfg->stepper != B200ADJ_ST_TSIT5_FIXED && !ros) { g_create_error = "stepper not built on device yet"; return B200ADJ_ERR_UNSUPPORTED; }
-        if (ros && !dense_fixed && !(cfg->abstol > 0 && cfg->reltol > 0)) { g_create_error = "adaptive steppers need abstol, reltol > 0"; return B200ADJ_ERR_INVALID; }
-        if (ros && mlp) { g_create_error = "MLP family: fixed-step Tsit5 only"; return B200ADJ_ERR_UNSUPPORTED; }
-    }
+    if (sde && m == 0) { g_create_error = "SDE stepper needs an SDE family"; return B200ADJ_ERR_INVALID; }
+    if (!sde && m != 0) { g_create_error = "ODE stepper with an SDE family"; return B200ADJ_ERR_INVALID; }
+    if (int32_t rc = support(SR_SENSEALG)) return rc;
+    if (!sde && cfg->stepper != B200ADJ_ST_TSIT5_FIXED && !ros) { g_create_error = "stepper not built on device yet"; return B200ADJ_ERR_UNSUPPORTED; }
+    if (ros && !dense_fixed && !(cfg->abstol > 0 && cfg->reltol > 0)) { g_create_error = "adaptive steppers need abstol, reltol > 0"; return B200ADJ_ERR_INVALID; }
     if (cfg->rhs_family == B200ADJ_FAM_RELAX && !t5a) { g_create_error = "Relax family: Tsit5 on the per-member dense framework (adaptive, or fixed step with B200ADJ_FLAG_DENSE_FORWARD)"; return B200ADJ_ERR_UNSUPPORTED; }
     if (cfg->rhs_family == B200ADJ_FAM_BALL && !t5a) { g_create_error = "BouncingBall family: Tsit5 on the per-member dense framework (adaptive, or fixed step with B200ADJ_FLAG_DENSE_FORWARD)"; return B200ADJ_ERR_UNSUPPORTED; }
+    int nsm = 132;
+    cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, cfg->device);
+    long long S = 0;                       // fixed grid: steps
+    std::vector<int32_t> sos;              // fixed grid: save index at grid point n, or -1
+    int maxs = 0, block = cfg->block_threads;
     if (ros) {
-        // adaptive path: save times are arbitrary ascending points of [t0, t1] (tstops of the reverse solve)
+        // per-member framework: save times are arbitrary ascending points of [t0, t1] (tstops of the reverse solve)
         for (int k = 0; k < cfg->K; k++) {
             if (cfg->saveat[k] < cfg->t0 || cfg->saveat[k] > cfg->t1 || (k > 0 && !(cfg->saveat[k] > cfg->saveat[k - 1]))) {
                 g_create_error = "saveat must be ascending inside [t0, t1]"; return B200ADJ_ERR_INVALID; }
         }
-        Handle* h = new Handle();
-        h->cfg = *cfg; h->cfg.m = 0; h->adaptive = true; h->nk = t5a ? 7 : 2; h->fixed_dt = dense_fixed;
-        h->saveat.assign(cfg->saveat, cfg->saveat + cfg->K);
-        h->cfg.saveat = h->saveat.data();
-        h->maxs = cfg->max_steps > 0 ? cfg->max_steps : 4096;      // per-member step capacity (forward and dense reverse)
+        maxs = cfg->max_steps > 0 ? cfg->max_steps : 4096;      // per-member step capacity (forward and dense reverse)
         if (dense_fixed) {
             // constant step: S forward steps; the reverse solve adds at most one clipped step per tstop (save times, events)
             const long long S_ = llround((cfg->t1 - cfg->t0) / cfg->dt);
             if (S_ < 1 || fabs(S_ * cfg->dt - (cfg->t1 - cfg->t0)) > 1e-9 * fmax(1.0, fabs(cfg->t1 - cfg->t0))) {
-                g_create_error = "(t1-t0) is not a whole number of dt steps"; delete h; return B200ADJ_ERR_UNSUPPORTED; }
+                g_create_error = "(t1-t0) is not a whole number of dt steps"; return B200ADJ_ERR_UNSUPPORTED; }
             const long long need = S_ + cfg->K + 64;
-            if (h->maxs < need) h->maxs = (int)(((need + 31) / 32) * 32);
+            if (maxs < need) maxs = (int)(((need + 31) / 32) * 32);
         }
-        h->block = cfg->block_threads ? cfg->block_threads : 128;
-        if (h->block < 32 || h->block > 256 || (h->block % 32)) { g_create_error = "block_threads must be a multiple of 32 in [32, 256] for Rosenbrock23"; delete h; return B200ADJ_ERR_INVALID; }
-        h->grid = (int)((cfg->N + h->block - 1) / h->block);
-#define CREATE_TRY(expr)                                                                         \
-        do { cudaError_t _e = (expr); if (_e != cudaSuccess) {                                   \
-            g_create_error = std::string(#expr) + ": " + cudaGetErrorString(_e);                 \
-            int32_t rc = (_e == cudaErrorMemoryAllocation) ? B200ADJ_ERR_OOM : B200ADJ_ERR_CUDA; \
-            free_all(h); delete h; return rc; } } while (0)
-        CREATE_TRY(cudaSetDevice(cfg->device));
-        CREATE_TRY(cudaStreamCreateWithFlags(&h->own_stream, cudaStreamNonBlocking));
-        h->stream = h->own_stream;
-        const size_t N = (size_t)cfg->N, MS = (size_t)h->maxs, e = sizeof(double);
-        if (t5a) {      // member-major records (u_n, k1..k7, t_n, h, 1/h, t_{n+1}) and knots: tsit5_adaptive.cuh
-            CREATE_TRY(cudaMalloc(&h->r_ftT, N * (MS + 1) * e));
-            CREATE_TRY(cudaMalloc(&h->r_frecT, N * (MS + 1) * (size_t)(8 * d + 4) * e));
-        } else {
-            CREATE_TRY(cudaMalloc(&h->r_ft, (MS + 1) * N * e));
-            CREATE_TRY(cudaMalloc(&h->r_fu, (MS + 1) * d * N * e));
-            CREATE_TRY(cudaMalloc(&h->r_fk, MS * h->nk * d * N * e));
+        if (block == 0) block = 128;
+        if (block < 32 || block > 256 || (block % 32)) { g_create_error = "block_threads must be a multiple of 32 in [32, 256] for Rosenbrock23"; return B200ADJ_ERR_INVALID; }
+    } else {
+        // fixed-step grid: the horizon must be a whole number of steps and every save time must be a grid point.
+        // (Off-grid tstops split a step in the reference; that case is delegated back to the reference path.)
+        const double span = cfg->t1 - cfg->t0;
+        S = llround(span / cfg->dt);
+        if (S < 1 || S > 2000000000LL || fabs(S * cfg->dt - span) > 1e-9 * fmax(1.0, fabs(span))) {
+            g_create_error = "(t1-t0) is not a whole number of dt steps"; return B200ADJ_ERR_UNSUPPORTED; }
+        sos.assign((size_t)S + 1, -1);
+        for (int k = 0; k < cfg->K; k++) {
+            const double tk = cfg->saveat[k];
+            const long long n = llround((tk - cfg->t0) / cfg->dt);
+            if (n < 0 || n > S || fabs(cfg->t0 + n * cfg->dt - tk) > 1e-9 * fmax(1.0, fabs(tk))) {
+                g_create_error = "saveat entry is not on the dt grid"; return B200ADJ_ERR_UNSUPPORTED; }
+            if (sos[n] != -1) { g_create_error = "duplicate save times are not supported"; return B200ADJ_ERR_UNSUPPORTED; }
+            if (k > 0 && !(tk > cfg->saveat[k - 1])) { g_create_error = "saveat must be ascending"; return B200ADJ_ERR_INVALID; }
+            sos[n] = k;
         }
-        CREATE_TRY(cudaMalloc(&h->r_fn, N * sizeof(int32_t)));
-        CREATE_TRY(cudaMalloc(&h->r_rn, N * sizeof(int32_t)));
-        h->maxseg = 2 * h->maxs;                                              // quadgk segment capacity per data interval (multiple of 32)
-        {
-            cudaDeviceGetAttribute(&h->nsm, cudaDevAttrMultiProcessorCount, cfg->device);
-            h->qgrid = quad_grid(cfg->N, h->nsm);
+        // Block size.  The reverse kernel is capped at 128 registers => at most 512 resident threads per SM; every thread
+        // runs the whole time loop, so the grid must fit in whole waves.  Default: ONE block per SM (block-wide barriers
+        // every few steps keep all warps of an SM in lockstep -- independent small blocks drift apart by >2x under the
+        // highest-warp-id-first arbiter and the stragglers run the tail latency-bound), sized so that the blocks cover
+        // the SMs evenly: block = ceil32(N / (nSM * waves)).
+        if (block == 0) {
+            const long long waves = (cfg->N + (long long)nsm * 512 - 1) / ((long long)nsm * 512);
+            long long per = (cfg->N + nsm * waves - 1) / (nsm * waves);
+            block = (int)(((per + 31) / 32) * 32);
+            if (block < 32) block = 32;
+            if (block > 512) block = 512;
         }
-        CREATE_TRY(cudaMalloc(&h->d_saveat, (size_t)(cfg->K > 0 ? cfg->K : 1) * e));
-        if (cfg->K > 0) CREATE_TRY(cudaMemcpy(h->d_saveat, cfg->saveat, (size_t)cfg->K * e, cudaMemcpyHostToDevice));
-        // the forward pass keeps its own save table: set_reverse_options may re-target the reverse pass' jump times
-        h->fwd_K = cfg->K; h->fwd_saveat = h->saveat;
-        CREATE_TRY(cudaMalloc(&h->d_fwd_saveat, (size_t)(cfg->K > 0 ? cfg->K : 1) * e));
-        if (cfg->K > 0) CREATE_TRY(cudaMemcpy(h->d_fwd_saveat, cfg->saveat, (size_t)cfg->K * e, cudaMemcpyHostToDevice));
-        h->qpartials_blocks = (size_t)h->qgrid + 1;                              // quadrature kernel: persistent grid
-        {   // block partials of the dG/dp reduction: the reverse kernels may run with blocks as small as one warp (disp_t5a.inc)
-            const size_t gmax = (size_t)((cfg->N + 31) / 32);
-            CREATE_TRY(cudaMalloc(&h->d_partials, (h->qpartials_blocks > gmax ? h->qpartials_blocks : gmax) * P * sizeof(double)));
+        if (block < 32 || block > 512 || (block % 32) != 0) { g_create_error = "block_threads must be a multiple of 32 in [32, 512]"; return B200ADJ_ERR_INVALID; }
+        if (mlp) block = MLP_TB;      // members per block (the kernels run MLP_THREADS threads per block)
+        if (ckpt_every > 1) {
+            if (int32_t rc = support(SR_CKPT)) return rc;
+            if (ckpt_every > S) ckpt_every = (int)S;
+            const size_t need = (size_t)ckpt_every * d * block * esz(*cfg);
+            if (need > 160 * 1024) { g_create_error = "checkpoint_every * d * block_threads * sizeof(real) exceeds 160 KB of shared memory: lower checkpoint_every or block_threads"; return B200ADJ_ERR_INVALID; }
         }
-        CREATE_TRY(cudaMalloc(&h->d_ticket, sizeof(unsigned int)));
-        CREATE_TRY(cudaMemset(h->d_ticket, 0, sizeof(unsigned int)));
-        if (!cfg->buffers_on_device) {
-            const size_t pn = cfg->shared_p ? (size_t)P : (size_t)P * N;
-            CREATE_TRY(cudaMalloc(&h->s_u0, d * N * e));
-            CREATE_TRY(cudaMalloc(&h->s_p, pn * e));
-            CREATE_TRY(cudaMalloc(&h->s_du0, d * N * e));
-            CREATE_TRY(cudaMalloc(&h->s_dp, pn * e));
-            CREATE_TRY(cudaMalloc(&h->s_status, N * sizeof(int32_t)));
-            if (cfg->K > 0) {
-                CREATE_TRY(cudaMalloc(&h->s_saved, (size_t)cfg->K * d * N * e));
-                if (cfg->cost_kind == B200ADJ_COST_EXPLICIT) CREATE_TRY(cudaMalloc(&h->s_dLdu, (size_t)cfg->K * d * N * e));
-            }
-        }
-#undef CREATE_TRY
-        for (int j = 0; j < 4; j++) { h->cost_av[j] = cfg->cost_a; h->cost_bv[j] = cfg->cost_b; }
-        *handle = h;
-        return B200ADJ_OK;
-    }
-    // fixed-step grid: the horizon must be a whole number of steps and every save time must be a grid point.
-    // (Off-grid tstops split a step in the reference; that case is delegated back to the reference path.)
-    const double span = cfg->t1 - cfg->t0;
-    const double Sf = span / cfg->dt;
-    const long long S = llround(Sf);
-    if (S < 1 || S > 2000000000LL || fabs(S * cfg->dt - span) > 1e-9 * fmax(1.0, fabs(span))) {
-        g_create_error = "(t1-t0) is not a whole number of dt steps"; return B200ADJ_ERR_UNSUPPORTED; }
-    std::vector<int32_t> sos((size_t)S + 1, -1);
-    for (int k = 0; k < cfg->K; k++) {
-        const double tk = cfg->saveat[k];
-        const long long n = llround((tk - cfg->t0) / cfg->dt);
-        if (n < 0 || n > S || fabs(cfg->t0 + n * cfg->dt - tk) > 1e-9 * fmax(1.0, fabs(tk))) {
-            g_create_error = "saveat entry is not on the dt grid"; return B200ADJ_ERR_UNSUPPORTED; }
-        if (sos[n] != -1) { g_create_error = "duplicate save times are not supported"; return B200ADJ_ERR_UNSUPPORTED; }
-        if (k > 0 && !(tk > cfg->saveat[k - 1])) { g_create_error = "saveat must be ascending"; return B200ADJ_ERR_INVALID; }
-        sos[n] = k;
-    }
-    // Block size.  The reverse kernel is capped at 128 registers => at most 512 resident threads per SM; every thread
-    // runs the whole time loop, so the grid must fit in whole waves.  Default: ONE block per SM (block-wide barriers
-    // every few steps keep all warps of an SM in lockstep -- independent small blocks drift apart by >2x under the
-    // highest-warp-id-first arbiter and the stragglers run the tail latency-bound), sized so that the blocks cover
-    // the SMs evenly: block = ceil32(N / (nSM * waves)).
-    int nsm = 132;
-    cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, cfg->device);
-    int block = cfg->block_threads;
-    if (block == 0) {
-        const long long waves = (cfg->N + (long long)nsm * 512 - 1) / ((long long)nsm * 512);
-        long long per = (cfg->N + nsm * waves - 1) / (nsm * waves);
-        block = (int)(((per + 31) / 32) * 32);
-        if (block < 32) block = 32;
-        if (block > 512) block = 512;
-    }
-    if (block < 32 || block > 512 || (block % 32) != 0) { g_create_error = "block_threads must be a multiple of 32 in [32, 512]"; return B200ADJ_ERR_INVALID; }
-    if (mlp) block = MLP_TB;      // members per block (the kernels run MLP_THREADS threads per block)
-    // interval checkpointing (a14): forward states every C steps, segments re-solved by the reverse kernel
-    int ckpt_every = cfg->checkpoint_every > 1 ? cfg->checkpoint_every : 1;
-    if (ckpt_every > 1) {
-        if (mlp || sde || (cfg->sensealg != B200ADJ_SA_INTERPOLATING && cfg->sensealg != B200ADJ_SA_GAUSS)) {
-            g_create_error = "checkpoint_every > 1: fixed-step Tsit5 with InterpolatingAdjoint / GaussAdjoint (the sensealgs that checkpoint in the reference)"; return B200ADJ_ERR_UNSUPPORTED; }
-        if (ckpt_every > S) ckpt_every = (int)S;
-        const size_t need = (size_t)ckpt_every * d * block * esz(*cfg);
-        if (need > 160 * 1024) { g_create_error = "checkpoint_every * d * block_threads * sizeof(real) exceeds 160 KB of shared memory: lower checkpoint_every or block_threads"; return B200ADJ_ERR_INVALID; }
     }
 
     Handle* h = new Handle();
-    h->cfg = *cfg; h->cfg.m = m;
+    h->cfg = *cfg; h->cfg.m = m; h->path = path;
     h->saveat.assign(cfg->saveat, cfg->saveat + cfg->K);
     h->cfg.saveat = h->saveat.data();
-    h->save_of_step = sos;
-    h->S = (int)S; h->block = block; h->ckpt_every = ckpt_every;
+    h->S = (int)S; h->maxs = maxs; h->block = block; h->ckpt_every = ckpt_every;
     h->grid = (int)((cfg->N + block - 1) / block);
+    h->nsm = nsm; h->qgrid = quad_grid(cfg->N, nsm);
+    h->qpartials_blocks = (size_t)h->qgrid + 1;                              // quadrature kernels: persistent grid
+    h->maxseg = ros ? 2 * maxs : 4096;                                       // quadgk segment capacity per data interval (multiple of 32)
 #define CREATE_TRY(expr)                                                                         \
     do { cudaError_t _e = (expr); if (_e != cudaSuccess) {                                       \
         g_create_error = std::string(#expr) + ": " + cudaGetErrorString(_e);                     \
@@ -411,43 +417,47 @@ int32_t b200adj_create(const b200adj_cfg* cfg, void** handle) {
     CREATE_TRY(cudaStreamCreateWithFlags(&h->own_stream, cudaStreamNonBlocking));
     h->stream = h->own_stream;
     const size_t N = (size_t)cfg->N, e = esz(*cfg);
-    const size_t Npad = ((N + block - 1) / block) * block;     // padded checkpoint pitch (whole TMA rows per block)
-    h->Npad = (int64_t)Npad;
-    const size_t ckpt_rows = ckpt_every > 1 ? ((size_t)S + ckpt_every - 1) / ckpt_every + 1 : (size_t)S + 1;
-    CREATE_TRY(cudaMalloc(&h->d_ckpt, ckpt_rows * d * Npad * e));
-    h->nsm = nsm; h->qgrid = quad_grid(cfg->N, nsm);
-    h->qpart_blocks_fixed = (size_t)h->qgrid + 1;
-    CREATE_TRY(cudaMalloc(&h->d_partials, (h->qpart_blocks_fixed > (size_t)h->grid ? h->qpart_blocks_fixed : (size_t)h->grid) * P * sizeof(double)));
+    // the forward pass keeps its own save table: set_reverse_options may re-target the reverse pass' jump times
+    h->fwd_K = cfg->K; h->fwd_saveat = h->saveat;
+    CREATE_TRY(upload_table(&h->d_saveat, cfg->saveat, (size_t)cfg->K));
+    if (ros) {
+        const size_t MS = (size_t)maxs;
+        if (t5a) {      // member-major records (u_n, k1..k7, t_n, h, 1/h, t_{n+1}) and knots: tsit5_adaptive.cuh
+            CREATE_TRY(cudaMalloc(&h->r_ftT, N * (MS + 1) * e));
+            CREATE_TRY(cudaMalloc(&h->r_frecT, N * (MS + 1) * (size_t)(8 * d + 4) * e));
+        } else {        // Rosenbrock23: step-major knots, states and the 2 dense-output stages
+            CREATE_TRY(cudaMalloc(&h->r_ft, (MS + 1) * N * e));
+            CREATE_TRY(cudaMalloc(&h->r_fu, (MS + 1) * d * N * e));
+            CREATE_TRY(cudaMalloc(&h->r_fk, MS * 2 * d * N * e));
+        }
+        CREATE_TRY(cudaMalloc(&h->r_fn, N * sizeof(int32_t)));
+        CREATE_TRY(cudaMalloc(&h->r_rn, N * sizeof(int32_t)));
+        CREATE_TRY(upload_table(&h->d_fwd_saveat, cfg->saveat, (size_t)cfg->K));
+    } else {
+        const size_t Npad = ((N + block - 1) / block) * block;     // padded checkpoint pitch (whole TMA rows per block)
+        h->Npad = (int64_t)Npad;
+        const size_t ckpt_rows = ckpt_every > 1 ? ((size_t)S + ckpt_every - 1) / ckpt_every + 1 : (size_t)S + 1;
+        CREATE_TRY(cudaMalloc(&h->d_ckpt, ckpt_rows * d * Npad * e));
+        h->save_of_step = sos; h->fwd_save_of_step = sos;
+        CREATE_TRY(upload_table(&h->d_save_of_step, sos.data(), sos.size()));
+        CREATE_TRY(upload_table(&h->d_fwd_save_of_step, sos.data(), sos.size()));
+        if (sde) CREATE_TRY(cudaMalloc(&h->d_noise, (size_t)S * m * N * e));
+        // BF16_F32ACC = mlp_tc.cuh: member and gradient GEMMs in the time loop on wgmma, fp32 accumulators in registers
+        if (is_mlp_tc(h)) CREATE_TRY(cudaMalloc(&h->d_kst, (size_t)S * 14 * N * sizeof(float)));
+        if (cfg->flags & B200ADJ_FLAG_TRACE) {
+            CREATE_TRY(cudaMalloc(&h->d_trace, (size_t)h->grid * 3 * sizeof(unsigned long long)));
+            CREATE_TRY(cudaMemset(h->d_trace, 0, (size_t)h->grid * 3 * sizeof(unsigned long long)));
+        }
+        if (!sde) build_tsit5_tables(cfg->dt, &h->tb);
+    }
+    {   // block partials of the dG/dp reduction; the T5A / ROS reverse kernels may run with blocks as small as one warp (disp_t5a.inc)
+        const size_t blocks = ros ? (N + 31) / 32 : (size_t)h->grid;
+        CREATE_TRY(cudaMalloc(&h->d_partials, (h->qpartials_blocks > blocks ? h->qpartials_blocks : blocks) * P * sizeof(double)));
+    }
     CREATE_TRY(cudaMalloc(&h->d_ticket, sizeof(unsigned int)));
     CREATE_TRY(cudaMemset(h->d_ticket, 0, sizeof(unsigned int)));
-    CREATE_TRY(cudaMalloc(&h->d_save_of_step, ((size_t)S + 1) * sizeof(int32_t)));
-    CREATE_TRY(cudaMemcpy(h->d_save_of_step, sos.data(), ((size_t)S + 1) * sizeof(int32_t), cudaMemcpyHostToDevice));
-    // the forward pass keeps its own save table: set_reverse_options may re-target the reverse pass' jump times
-    h->fwd_K = cfg->K; h->fwd_saveat = h->saveat; h->fwd_save_of_step = sos;
-    CREATE_TRY(cudaMalloc(&h->d_fwd_save_of_step, ((size_t)S + 1) * sizeof(int32_t)));
-    CREATE_TRY(cudaMemcpy(h->d_fwd_save_of_step, sos.data(), ((size_t)S + 1) * sizeof(int32_t), cudaMemcpyHostToDevice));
-    if (sde) CREATE_TRY(cudaMalloc(&h->d_noise, (size_t)S * m * N * e));
-    // BF16_F32ACC = mlp_tc.cuh: member and gradient GEMMs in the time loop on wgmma, fp32 accumulators in registers
-    h->mlp_tc = mlp && cfg->dtype == B200ADJ_BF16_F32ACC;
-    if (h->mlp_tc) CREATE_TRY(cudaMalloc(&h->d_kst, (size_t)S * 14 * N * sizeof(float)));
-    if (cfg->flags & B200ADJ_FLAG_TRACE) {
-        CREATE_TRY(cudaMalloc(&h->d_trace, (size_t)h->grid * 3 * sizeof(unsigned long long)));
-        CREATE_TRY(cudaMemset(h->d_trace, 0, (size_t)h->grid * 3 * sizeof(unsigned long long)));
-    }
-    if (!cfg->buffers_on_device) {
-        const size_t pn = cfg->shared_p ? (size_t)P : (size_t)P * N;
-        CREATE_TRY(cudaMalloc(&h->s_u0, d * N * e));
-        CREATE_TRY(cudaMalloc(&h->s_p, pn * e));
-        CREATE_TRY(cudaMalloc(&h->s_du0, d * N * e));
-        CREATE_TRY(cudaMalloc(&h->s_dp, pn * e));
-        CREATE_TRY(cudaMalloc(&h->s_status, N * sizeof(int32_t)));
-        if (cfg->K > 0) {
-            CREATE_TRY(cudaMalloc(&h->s_saved, (size_t)cfg->K * d * N * e));
-            if (cfg->cost_kind == B200ADJ_COST_EXPLICIT) CREATE_TRY(cudaMalloc(&h->s_dLdu, (size_t)cfg->K * d * N * e));
-        }
-    }
+    if (!cfg->buffers_on_device) CREATE_TRY(alloc_staging(h));
 #undef CREATE_TRY
-    if (!sde) build_tsit5_tables(cfg->dt, &h->tb);
     for (int j = 0; j < 4; j++) { h->cost_av[j] = cfg->cost_a; h->cost_bv[j] = cfg->cost_b; }
     *handle = h;
     return B200ADJ_OK;
@@ -459,54 +469,37 @@ int32_t b200adj_set_reverse_options(void* handle, int32_t sensealg, int32_t cost
     Handle* h = (Handle*)handle;
     b200adj_cfg& c = h->cfg;
     if (sensealg < 0 || sensealg > 4 || (cost_kind != B200ADJ_COST_EXPLICIT && cost_kind != B200ADJ_COST_AFFINE)) { h->err = "bad sensealg/cost_kind"; return B200ADJ_ERR_INVALID; }
-    if (h->cc_on && sensealg == B200ADJ_SA_QUADRATURE) { h->err = "continuous callback: QuadratureAdjoint has no callback support"; return B200ADJ_ERR_UNSUPPORTED; }
-    if (sensealg == B200ADJ_SA_GAUSSKRONROD && (is_sde(c) || c.rhs_family == B200ADJ_FAM_MLP || c.dtype != B200ADJ_F64)) { h->err = "GaussKronrodAdjoint: F64, named ODE families"; return B200ADJ_ERR_UNSUPPORTED; }
-    if (h->ckpt_every > 1 && sensealg != B200ADJ_SA_INTERPOLATING && sensealg != B200ADJ_SA_GAUSS) { h->err = "checkpoint_every > 1: InterpolatingAdjoint / GaussAdjoint only"; return B200ADJ_ERR_UNSUPPORTED; }
-    if (is_sde(c) && sensealg != B200ADJ_SA_BACKSOLVE && sensealg != B200ADJ_SA_INTERPOLATING) { h->err = "SDE: BacksolveAdjoint / InterpolatingAdjoint are built"; return B200ADJ_ERR_UNSUPPORTED; }
-    if (c.rhs_family == B200ADJ_FAM_MLP && sensealg != B200ADJ_SA_INTERPOLATING && sensealg != B200ADJ_SA_GAUSS) { h->err = "MLP family: InterpolatingAdjoint / GaussAdjoint are built"; return B200ADJ_ERR_UNSUPPORTED; }
-    if (h->nev > 0 && sensealg == B200ADJ_SA_QUADRATURE) { h->err = "events: QuadratureAdjoint has no callback support"; return B200ADJ_ERR_UNSUPPORTED; }
-    if (c.dtype == B200ADJ_F32 && c.rhs_family != B200ADJ_FAM_MLP && sensealg == B200ADJ_SA_QUADRATURE) { h->err = "F32: QuadratureAdjoint is F64 only"; return B200ADJ_ERR_UNSUPPORTED; }
+    if (int32_t rc = check_support(h, sensealg, h->nev > 0, h->cc_on)) return rc;
     CUDA_TRY(h, cudaSetDevice(c.device));
-    if (h->adaptive) {
-        if (K >= 0) {
-            for (int k = 0; k < K; k++)
-                if (t[k] < c.t0 || t[k] > c.t1 || (k > 0 && !(t[k] > t[k - 1]))) { h->err = "t must be ascending inside [t0, t1]"; return B200ADJ_ERR_INVALID; }
-            CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-            if (K > c.K) { cudaFree(h->d_saveat); h->d_saveat = nullptr; CUDA_TRY(h, cudaMalloc(&h->d_saveat, (size_t)K * sizeof(double))); cudaFree(h->s_dLdu); h->s_dLdu = nullptr; }
-            if (K > 0) CUDA_TRY(h, cudaMemcpy(h->d_saveat, t, (size_t)K * sizeof(double), cudaMemcpyHostToDevice));
-            h->saveat.assign(t, t + K); c.saveat = h->saveat.data(); c.K = K;
-        }
-        if (!c.buffers_on_device && cost_kind == B200ADJ_COST_EXPLICIT && c.K > 0 && !h->s_dLdu)
-            CUDA_TRY(h, cudaMalloc(&h->s_dLdu, (size_t)c.K * c.d * (size_t)c.N * esz(c)));
-        c.sensealg = sensealg; c.cost_kind = cost_kind; c.cost_a = cost_a; c.cost_b = cost_b;
-        for (int j = 0; j < 4; j++) { h->cost_av[j] = cost_a; h->cost_bv[j] = cost_b; }
-        h->has_dgdp = false;
-        c.flags = (c.flags & B200ADJ_CREATE_FLAGS) | (flags & ~B200ADJ_CREATE_FLAGS);
-        return B200ADJ_OK;
-    }
     if (K >= 0) {
         if (K > 0 && !t) { h->err = "null t"; return B200ADJ_ERR_INVALID; }
-        std::vector<int32_t> sos((size_t)h->S + 1, -1);
-        for (int k = 0; k < K; k++) {
-            const long long n = llround((t[k] - c.t0) / c.dt);
-            if (n < 0 || n > h->S || fabs(c.t0 + n * c.dt - t[k]) > 1e-9 * fmax(1.0, fabs(t[k]))) { h->err = "t entry is not on the dt grid"; return B200ADJ_ERR_UNSUPPORTED; }
-            if (sos[n] != -1) { h->err = "duplicate save times are not supported"; return B200ADJ_ERR_UNSUPPORTED; }
-            sos[n] = k;
+        std::vector<int32_t> sos;
+        if (is_adaptive(h)) {
+            for (int k = 0; k < K; k++)
+                if (t[k] < c.t0 || t[k] > c.t1 || (k > 0 && !(t[k] > t[k - 1]))) { h->err = "t must be ascending inside [t0, t1]"; return B200ADJ_ERR_INVALID; }
+        } else {
+            sos.assign((size_t)h->S + 1, -1);
+            for (int k = 0; k < K; k++) {
+                const long long n = llround((t[k] - c.t0) / c.dt);
+                if (n < 0 || n > h->S || fabs(c.t0 + n * c.dt - t[k]) > 1e-9 * fmax(1.0, fabs(t[k]))) { h->err = "t entry is not on the dt grid"; return B200ADJ_ERR_UNSUPPORTED; }
+                if (sos[n] != -1) { h->err = "duplicate save times are not supported"; return B200ADJ_ERR_UNSUPPORTED; }
+                sos[n] = k;
+            }
         }
         CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-        CUDA_TRY(h, cudaMemcpy(h->d_save_of_step, sos.data(), sos.size() * sizeof(int32_t), cudaMemcpyHostToDevice));
-        h->save_of_step = sos;
-        h->saveat.assign(t, t + K);
-        c.saveat = h->saveat.data();
-        if (!c.buffers_on_device && K > c.K) {
+        if (!sos.empty()) {
+            CUDA_TRY(h, cudaMemcpy(h->d_save_of_step, sos.data(), sos.size() * sizeof(int32_t), cudaMemcpyHostToDevice));
+            h->save_of_step = sos;
+        }
+        if (K > c.K) {
+            cudaFree(h->d_saveat); h->d_saveat = nullptr; CUDA_TRY(h, cudaMalloc(&h->d_saveat, (size_t)K * sizeof(double)));
             cudaFree(h->s_dLdu); h->s_dLdu = nullptr;
         }
-        if (!c.buffers_on_device && cost_kind == B200ADJ_COST_EXPLICIT && K > 0 && !h->s_dLdu)
-            CUDA_TRY(h, cudaMalloc(&h->s_dLdu, (size_t)K * c.d * (size_t)c.N * esz(c)));
-        c.K = K;
-    } else if (!c.buffers_on_device && cost_kind == B200ADJ_COST_EXPLICIT && c.K > 0 && !h->s_dLdu) {
-        CUDA_TRY(h, cudaMalloc(&h->s_dLdu, (size_t)c.K * c.d * (size_t)c.N * esz(c)));
+        if (K > 0) CUDA_TRY(h, cudaMemcpy(h->d_saveat, t, (size_t)K * sizeof(double), cudaMemcpyHostToDevice));
+        h->saveat.assign(t, t + K); c.saveat = h->saveat.data(); c.K = K;
     }
+    if (!c.buffers_on_device && cost_kind == B200ADJ_COST_EXPLICIT && c.K > 0 && !h->s_dLdu)
+        CUDA_TRY(h, cudaMalloc(&h->s_dLdu, (size_t)c.K * c.d * (size_t)c.N * esz(c)));
     c.sensealg = sensealg; c.cost_kind = cost_kind; c.cost_a = cost_a; c.cost_b = cost_b;
     for (int j = 0; j < 4; j++) { h->cost_av[j] = cost_a; h->cost_bv[j] = cost_b; }
     h->has_dgdp = false;
@@ -517,7 +510,7 @@ int32_t b200adj_set_reverse_options(void* handle, int32_t sensealg, int32_t cost
 int32_t b200adj_set_continuous_cost(void* handle, int32_t enabled, double a, double b) {
     if (!handle) return B200ADJ_ERR_INVALID;
     Handle* h = (Handle*)handle;
-    if (enabled && ((h->adaptive && h->cfg.stepper != B200ADJ_ST_TSIT5_ADAPTIVE && !h->fixed_dt) || is_sde(h->cfg) || h->cfg.rhs_family == B200ADJ_FAM_MLP)) {
+    if (enabled && h->path != Path::FIXED && h->path != Path::T5A) {
         h->err = "continuous cost: built for the Tsit5 ODE paths (fixed step and adaptive)"; return B200ADJ_ERR_UNSUPPORTED; }
     h->cont_on = enabled != 0;
     for (int j = 0; j < 4; j++) { h->cont_av[j] = a; h->cont_bv[j] = b; }
@@ -544,7 +537,7 @@ int32_t b200adj_register_family(const char* plugin_path, int32_t* family_id) {
 }
 
 int32_t b200adj_family_info(int32_t family_id, int32_t* d, int32_t* P, const char** name) {
-    const FamilyVTable* vt = family_lookup(family_id);
+    const FamilyVTable* vt = family_id >= B200ADJ_FAM_USER_BASE_ID ? family_lookup(family_id) : nullptr;     // registered plug-ins
     if (!vt) return B200ADJ_ERR_INVALID;
     if (d) *d = vt->d;
     if (P) *P = vt->P;
@@ -578,9 +571,9 @@ int32_t b200adj_set_events(void* handle, int32_t E, const double* times, const d
     if (E < 0 || (E > 0 && (!times || !scale || !shift)) || ((pscale == nullptr) != (pshift == nullptr))) { h->err = "set_events: bad arguments"; return B200ADJ_ERR_INVALID; }
     if (E > 0 && h->cc_on) { h->err = "events: preset-time events together with a continuous callback are not built"; return B200ADJ_ERR_UNSUPPORTED; }
     // hybrid neural ODE (test/Core5/HybridNODE.jl): the MLP family's CUDA-core kernels (F64 / F32) carry state events on the dt grid
-    const bool mlp_ev = c.rhs_family == B200ADJ_FAM_MLP && !h->mlp_tc && c.stepper == B200ADJ_ST_TSIT5_FIXED;
-    const bool fixed = c.stepper == B200ADJ_ST_TSIT5_FIXED && !h->fixed_dt && ((c.rhs_family != B200ADJ_FAM_MLP && c.dtype == B200ADJ_F64) || mlp_ev);
-    if (E > 0 && c.stepper != B200ADJ_ST_TSIT5_ADAPTIVE && !fixed && !h->fixed_dt) { h->err = "events: built for the Tsit5 steppers (adaptive; fixed step in F64; MLP family: F64 / F32, not the bf16 tensor-core path)"; return B200ADJ_ERR_UNSUPPORTED; }
+    const bool mlp_ev = h->path == Path::MLP && !is_mlp_tc(h);
+    const bool fixed = (h->path == Path::FIXED && c.dtype == B200ADJ_F64) || mlp_ev;     // events on the dt grid
+    if (E > 0 && h->path != Path::T5A && !fixed) { h->err = "events: built for the Tsit5 steppers (adaptive; fixed step in F64; MLP family: F64 / F32, not the bf16 tensor-core path)"; return B200ADJ_ERR_UNSUPPORTED; }
     if (E > 0 && mlp_ev && pscale) { h->err = "events: parameter-changing affects are not built for the MLP family"; return B200ADJ_ERR_UNSUPPORTED; }
     if (E > 0 && fixed && h->ckpt_every > 1) { h->err = "events together with checkpoint_every > 1 are not built"; return B200ADJ_ERR_UNSUPPORTED; }
     std::vector<int32_t> eos;
@@ -594,7 +587,7 @@ int32_t b200adj_set_events(void* handle, int32_t E, const double* times, const d
             eos[n] = e;
         }
     }
-    if (E > 0 && c.sensealg == B200ADJ_SA_QUADRATURE) { h->err = "events: Interpolating / Gauss / Backsolve (QuadratureAdjoint has no callback support)"; return B200ADJ_ERR_UNSUPPORTED; }
+    if (E > 0) if (int32_t rc = check_support(h, c.sensealg, true, h->cc_on)) return rc;
     for (int e = 0; e < E; e++)
         if (!(times[e] > c.t0 && times[e] < c.t1) || (e > 0 && !(times[e] > times[e - 1]))) { h->err = "events: times must be ascending and strictly inside (t0, t1)"; return B200ADJ_ERR_INVALID; }
     CUDA_TRY(h, cudaSetDevice(c.device));
@@ -635,7 +628,7 @@ int32_t b200adj_set_event_param_shift(void* handle, const int32_t* comp, const i
     h->have_forward = false;
     if (!comp) return B200ADJ_OK;                                      // removes the shifts
     if (!param || !coef) { h->err = "event parameter shift: null argument"; return B200ADJ_ERR_INVALID; }
-    if (!(c.stepper == B200ADJ_ST_TSIT5_ADAPTIVE || h->fixed_dt)) {
+    if (h->path != Path::T5A) {
         h->err = "event parameter shift: built on the per-member dense framework (adaptive Tsit5, or fixed step with B200ADJ_FLAG_DENSE_FORWARD)";
         return B200ADJ_ERR_UNSUPPORTED; }
     for (int e = 0; e < h->nev; e++)
@@ -663,8 +656,8 @@ int32_t b200adj_set_continuous_callback(void* handle, int32_t enabled, int32_t i
         cudaFree(h->d_cc_t); cudaFree(h->d_cc_n); h->d_cc_t = nullptr; h->d_cc_n = nullptr; h->cc_on = false; h->have_forward = false;
         return B200ADJ_OK;
     }
-    if (c.stepper != B200ADJ_ST_TSIT5_ADAPTIVE || h->fixed_dt || c.dtype != B200ADJ_F64) { h->err = "continuous callback: built for the adaptive Tsit5 stepper (F64)"; return B200ADJ_ERR_UNSUPPORTED; }
-    if (c.sensealg == B200ADJ_SA_QUADRATURE) { h->err = "continuous callback: Interpolating / Gauss / GaussKronrod / Backsolve (QuadratureAdjoint has no callback support)"; return B200ADJ_ERR_UNSUPPORTED; }
+    if (h->path != Path::T5A || is_fixed_dt(h)) { h->err = "continuous callback: built for the adaptive Tsit5 stepper (F64)"; return B200ADJ_ERR_UNSUPPORTED; }
+    if (int32_t rc = check_support(h, c.sensealg, h->nev > 0, true)) return rc;
     if (h->nev > 0) { h->err = "continuous callback together with preset-time events is not built"; return B200ADJ_ERR_UNSUPPORTED; }
     if (c.d > 4) { h->err = "continuous callback: d <= 4"; return B200ADJ_ERR_UNSUPPORTED; }
     if (idx < 0 || idx >= c.d || direction < -1 || direction > 1 || pcomp >= c.d || (pcomp >= 0 && (pparam < 0 || pparam >= c.P)) || max_events < 1 ||
@@ -744,7 +737,7 @@ int64_t b200adj_launch_count(void* handle) { return handle ? ((Handle*)handle)->
 int32_t b200adj_get_step_counts(void* handle, int32_t* fwd_steps, int32_t* rev_steps) {
     if (!handle) return B200ADJ_ERR_INVALID;
     Handle* h = (Handle*)handle;
-    if (!h->adaptive) { h->err = "fixed-step handle: step count is S for every member"; return B200ADJ_ERR_UNSUPPORTED; }
+    if (!is_adaptive(h)) { h->err = "fixed-step handle: step count is S for every member"; return B200ADJ_ERR_UNSUPPORTED; }
     CUDA_TRY(h, cudaSetDevice(h->cfg.device));
     const cudaMemcpyKind kind = h->cfg.buffers_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
     if (fwd_steps) CUDA_TRY(h, cudaMemcpyAsync(fwd_steps, h->r_fn, (size_t)h->cfg.N * sizeof(int32_t), kind, h->stream));
@@ -772,54 +765,31 @@ int32_t b200adj_forward(void* handle, const void* u0, const void* p, const void*
         dstatus = status ? h->s_status : nullptr;
     }
     h->cur_p = dp;
+    const FamilyVTable* vt = family_lookup(c.rhs_family);      // the ODE paths' launchers
     int rc = 0;
-    if (h->adaptive && (c.stepper == B200ADJ_ST_TSIT5_ADAPTIVE || h->fixed_dt)) {
-        T5aArgs a = t5a_args(h);
-        a.saveat = h->d_fwd_saveat; a.K = h->fwd_K;
-        a.u0 = du0; a.p = dp; a.saved = h->fwd_K > 0 ? dsaved : nullptr; a.status = dstatus;
-        switch (c.rhs_family) {
-        case B200ADJ_FAM_LV: rc = launch_t5a_fwd<LotkaVolterra>(h, a); break;
-        case B200ADJ_FAM_LORENZ: rc = launch_t5a_fwd<Lorenz>(h, a); break;
-        case B200ADJ_FAM_ROBERTSON: rc = launch_t5a_fwd<Robertson>(h, a); break;
-        case B200ADJ_FAM_BALL: rc = launch_t5a_fwd<BouncingBall>(h, a); break;
-        case B200ADJ_FAM_RELAX: rc = launch_t5a_fwd<Relax>(h, a); break;
-        default: { const FamilyVTable* vt = family_lookup(c.rhs_family); rc = (vt && vt->t5a_fwd) ? vt->t5a_fwd(h, a) : B200ADJ_ERR_UNSUPPORTED; }
-        }
-    } else if (h->adaptive) {
-        RosArgs a = ros_args(h);
-        a.saveat = h->d_fwd_saveat; a.K = h->fwd_K;
-        a.u0 = du0; a.p = dp; a.saved = h->fwd_K > 0 ? dsaved : nullptr; a.status = dstatus;
-        switch (c.rhs_family) {
-        case B200ADJ_FAM_LV: rc = launch_ros_fwd<LotkaVolterra>(h, a); break;
-        case B200ADJ_FAM_LORENZ: rc = launch_ros_fwd<Lorenz>(h, a); break;
-        case B200ADJ_FAM_ROBERTSON: rc = launch_ros_fwd<Robertson>(h, a); break;
-        default: { const FamilyVTable* vt = family_lookup(c.rhs_family); rc = (vt && vt->ros_fwd) ? vt->ros_fwd(h, a) : B200ADJ_ERR_UNSUPPORTED; }
-        }
-    } else if (c.rhs_family == B200ADJ_FAM_MLP) {
+    if (is_adaptive(h)) {
+        auto fwd = [&](auto a, auto fn) {
+            a.saveat = h->d_fwd_saveat; a.K = h->fwd_K;
+            a.u0 = du0; a.p = dp; a.saved = h->fwd_K > 0 ? dsaved : nullptr; a.status = dstatus;
+            return launch(fn, h, a);
+        };
+        rc = h->path == Path::T5A ? fwd(t5a_args(h), vt->t5a_fwd) : fwd(dense_args<RosArgs>(h), vt->ros_fwd);
+    } else if (h->path == Path::MLP) {
         rc = mlp_forward_dispatch(h, du0, dp, h->fwd_K > 0 ? dsaved : nullptr, dstatus);
-    } else if (!is_sde(c) && c.dtype == B200ADJ_F32) {
+    } else if (h->path == Path::FIXED && c.dtype == B200ADJ_F32) {
         OdeFwdArgsT<float> a;
         memset(&a, 0, sizeof(a));
         a.u0 = (const float*)du0; a.p = (const float*)dp; a.ckpt = (float*)h->d_ckpt; a.saved = h->fwd_K > 0 ? (float*)dsaved : nullptr;
         a.save_of_step = h->d_fwd_save_of_step; a.status = dstatus; a.N = c.N; a.Npad = h->Npad; a.S = h->S; a.ckpt_every = h->ckpt_every;
         cast_tables(h->tb, &a.tb);
-        switch (c.rhs_family) {
-        case B200ADJ_FAM_LV: rc = launch_fwd_f32<LotkaVolterra>(h, a); break;
-        case B200ADJ_FAM_LORENZ: rc = launch_fwd_f32<Lorenz>(h, a); break;
-        default: rc = B200ADJ_ERR_UNSUPPORTED;
-        }
-    } else if (!is_sde(c)) {
+        rc = launch(vt->fwd_f32, h, a);
+    } else if (h->path == Path::FIXED) {
         OdeFwdArgs a;
         memset(&a, 0, sizeof(a));
         a.u0 = du0; a.p = dp; a.ckpt = h->d_ckpt; a.saved = h->fwd_K > 0 ? dsaved : nullptr; a.save_of_step = h->d_fwd_save_of_step;
         a.status = dstatus; a.N = c.N; a.Npad = h->Npad; a.S = h->S; a.tb = h->tb; a.ckpt_every = h->ckpt_every;
         a.event_of_step = h->d_event_of_step; a.ev_s = h->d_ev_s; a.ev_c = h->d_ev_c; a.ev_ps = h->d_ev_ps; a.ev_pc = h->d_ev_pc; a.nev = h->nev;
-        switch (c.rhs_family) {
-        case B200ADJ_FAM_LV: rc = launch_fwd<LotkaVolterra>(h, a); break;
-        case B200ADJ_FAM_LORENZ: rc = launch_fwd<Lorenz>(h, a); break;
-        case B200ADJ_FAM_ROBERTSON: rc = launch_fwd<Robertson>(h, a); break;
-        default: { const FamilyVTable* vt = family_lookup(c.rhs_family); rc = (vt && vt->fwd) ? vt->fwd(h, a) : B200ADJ_ERR_UNSUPPORTED; }
-        }
+        rc = launch(vt->fwd, h, a);
     } else {
         SdeFwdArgs a;
         a.u0 = du0; a.p = dp; a.ckpt = h->d_ckpt; a.saved = h->fwd_K > 0 ? dsaved : nullptr; a.save_of_step = h->d_fwd_save_of_step;
@@ -871,33 +841,18 @@ int32_t b200adj_reverse(void* handle, const void* dLdu, void* du0, void* dp) {
     }
     int rc = 0;
     bool fused_allreduce = false;
-    if (h->adaptive && (c.stepper == B200ADJ_ST_TSIT5_ADAPTIVE || h->fixed_dt)) {
-        T5aArgs a = t5a_args(h);
-        a.p = h->cur_p; a.dLdu = dL; a.du0 = ddu0; a.dp_members = ddp; a.dp = ddp;
-        if (h->adj_abstol > 0) a.abstol = h->adj_abstol;
-        if (h->adj_reltol > 0) a.reltol = h->adj_reltol;
-        switch (c.rhs_family) {
-        case B200ADJ_FAM_LV: rc = launch_t5a_rev<LotkaVolterra>(h, a); break;
-        case B200ADJ_FAM_LORENZ: rc = launch_t5a_rev<Lorenz>(h, a); break;
-        case B200ADJ_FAM_ROBERTSON: rc = launch_t5a_rev<Robertson>(h, a); break;
-        case B200ADJ_FAM_BALL: rc = launch_t5a_rev<BouncingBall>(h, a); break;
-        case B200ADJ_FAM_RELAX: rc = launch_t5a_rev<Relax>(h, a); break;
-        default: { const FamilyVTable* vt = family_lookup(c.rhs_family); rc = (vt && vt->t5a_rev) ? vt->t5a_rev(h, a) : B200ADJ_ERR_UNSUPPORTED; }
-        }
-    } else if (h->adaptive) {
-        RosArgs a = ros_args(h);
-        a.p = h->cur_p; a.dLdu = dL; a.du0 = ddu0; a.dp_members = ddp; a.dp = ddp;
-        if (h->adj_abstol > 0) a.abstol = h->adj_abstol;
-        if (h->adj_reltol > 0) a.reltol = h->adj_reltol;
-        switch (c.rhs_family) {
-        case B200ADJ_FAM_LV: rc = launch_ros_rev<LotkaVolterra>(h, a); break;
-        case B200ADJ_FAM_LORENZ: rc = launch_ros_rev<Lorenz>(h, a); break;
-        case B200ADJ_FAM_ROBERTSON: rc = launch_ros_rev<Robertson>(h, a); break;
-        default: { const FamilyVTable* vt = family_lookup(c.rhs_family); rc = (vt && vt->ros_rev) ? vt->ros_rev(h, a) : B200ADJ_ERR_UNSUPPORTED; }
-        }
-    } else if (c.rhs_family == B200ADJ_FAM_MLP) {
+    const FamilyVTable* vt = family_lookup(c.rhs_family);      // the ODE paths' launchers
+    if (is_adaptive(h)) {
+        auto rev = [&](auto a, auto fn) {
+            a.p = h->cur_p; a.dLdu = dL; a.du0 = ddu0; a.dp_members = ddp; a.dp = ddp;
+            if (h->adj_abstol > 0) a.abstol = h->adj_abstol;
+            if (h->adj_reltol > 0) a.reltol = h->adj_reltol;
+            return launch(fn, h, a);
+        };
+        rc = h->path == Path::T5A ? rev(t5a_args(h), vt->t5a_rev) : rev(dense_args<RosArgs>(h), vt->ros_rev);
+    } else if (h->path == Path::MLP) {
         rc = mlp_reverse_dispatch(h, dL, ddu0, ddp);
-    } else if (!is_sde(c) && c.dtype == B200ADJ_F32) {
+    } else if (h->path == Path::FIXED && c.dtype == B200ADJ_F32) {
         if (h->cont_on) { h->err = "continuous cost: F64 only"; return B200ADJ_ERR_UNSUPPORTED; }
         OdeRevArgsT<float> a;
         memset(&a, 0, sizeof(a));
@@ -906,14 +861,9 @@ int32_t b200adj_reverse(void* handle, const void* dLdu, void* du0, void* dp) {
         a.N = c.N; a.Npad = h->Npad; a.S = h->S; a.trace = h->d_trace;
         for (int j = 0; j < 4; j++) { a.cost_a[j] = (float)h->cost_av[j]; a.cost_b[j] = (float)h->cost_bv[j]; }
         cast_tables(h->tb, &a.tb);
-        a.flags = ((c.flags & B200ADJ_FLAG_NO_START) ? 1u : 0u) | ((c.flags & B200ADJ_FLAG_NO_CHECKPOINTING) ? 2u : 0u) |
-                  ((c.flags & B200ADJ_FLAG_CKPT_EVERY_STEP) ? 4u : 0u);
-        switch (c.rhs_family) {
-        case B200ADJ_FAM_LV: rc = launch_rev_f32<LotkaVolterra>(h, a); break;
-        case B200ADJ_FAM_LORENZ: rc = launch_rev_f32<Lorenz>(h, a); break;
-        default: rc = B200ADJ_ERR_UNSUPPORTED;
-        }
-    } else if (!is_sde(c)) {
+        a.flags = kernel_flags(h);
+        rc = launch(vt->rev_f32, h, a);
+    } else if (h->path == Path::FIXED) {
         OdeRevArgs a;
         memset(&a, 0, sizeof(a));
         a.event_of_step = h->d_event_of_step; a.ev_s = h->d_ev_s; a.ev_c = h->d_ev_c; a.ev_ps = h->d_ev_ps; a.ev_pc = h->d_ev_pc; a.nev = h->nev;
@@ -926,21 +876,15 @@ int32_t b200adj_reverse(void* handle, const void* dLdu, void* du0, void* dp) {
         a.du0 = ddu0; a.dp_members = ddp; a.partials = h->d_partials; a.dp = ddp; a.ticket = h->d_ticket;
         a.N = c.N; a.Npad = h->Npad; a.S = h->S; a.tb = h->tb; a.trace = h->d_trace;
         for (int j = 0; j < 4; j++) { a.cost_a[j] = h->cost_av[j]; a.cost_b[j] = h->cost_bv[j]; a.cont_a[j] = h->cont_av[j]; a.cont_b[j] = h->cont_bv[j]; }
-        a.flags = ((c.flags & B200ADJ_FLAG_NO_START) ? 1u : 0u) | ((c.flags & B200ADJ_FLAG_NO_CHECKPOINTING) ? 2u : 0u) |
-                  ((c.flags & B200ADJ_FLAG_CKPT_EVERY_STEP) ? 4u : 0u) | (h->cont_on ? 8u : 0u);
-        switch (c.rhs_family) {
-        case B200ADJ_FAM_LV: rc = launch_rev<LotkaVolterra>(h, a); break;
-        case B200ADJ_FAM_LORENZ: rc = launch_rev<Lorenz>(h, a); break;
-        case B200ADJ_FAM_ROBERTSON: rc = launch_rev<Robertson>(h, a); break;
-        default: { const FamilyVTable* vt = family_lookup(c.rhs_family); rc = (vt && vt->rev) ? vt->rev(h, a) : B200ADJ_ERR_UNSUPPORTED; }
-        }
+        a.flags = kernel_flags(h);
+        rc = launch(vt->rev, h, a);
     } else {
         SdeRevArgs a;
         a.ckpt = h->d_ckpt; a.p = h->cur_p; a.dLdu = dL; a.save_of_step = h->d_save_of_step;
         a.du0 = ddu0; a.dp_members = ddp; a.partials = h->d_partials; a.dp = ddp; a.ticket = h->d_ticket;
         a.N = c.N; a.S = h->S; a.h = c.dt;
         for (int j = 0; j < 4; j++) { a.cost_a[j] = h->cost_av[j]; a.cost_b[j] = h->cost_bv[j]; }
-        a.flags = ((c.flags & B200ADJ_FLAG_NO_START) ? 1u : 0u) | ((c.flags & B200ADJ_FLAG_NO_CHECKPOINTING) ? 2u : 0u) | ((c.flags & B200ADJ_FLAG_CKPT_EVERY_STEP) ? 4u : 0u);
+        a.flags = kernel_flags(h);
         a.seed = c.seed; a.traj_offset = c.traj_offset;
         a.noise = h->noise_valid ? h->d_noise : nullptr;
         rc = sde_reverse_dispatch(h, a);

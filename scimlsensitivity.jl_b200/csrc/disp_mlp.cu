@@ -42,7 +42,7 @@ int mlp_tc_reverse_launch(Handle* h, const void* dLdu, void* du0, void* dp) {
     memset(&a, 0, sizeof(a));
     a.p = (const float*)h->cur_p; a.ckpt = (float*)h->d_ckpt; a.save_of_step = h->d_save_of_step; a.dLdu = (const float*)dLdu;
     a.du0 = (float*)du0; a.partials = (float*)h->d_partials; a.dp = (float*)dp; a.N = c.N; a.S = h->S; a.tb = h->tb; a.kst = h->d_kst;
-    for (int j = 0; j < 4; j++) { a.cost_a[j] = h->cost_av[j]; a.cost_b[j] = h->cost_bv[j]; } a.flags = (c.flags & B200ADJ_FLAG_NO_START) ? 1u : 0u;
+    for (int j = 0; j < 4; j++) { a.cost_a[j] = h->cost_av[j]; a.cost_b[j] = h->cost_bv[j]; } a.flags = kernel_flags(h) & KF_NO_START;
     const bool narrow = mlp_tc_narrow(h), ex = c.cost_kind == B200ADJ_COST_EXPLICIT;
     const size_t smem = (narrow ? sizeof(TcSmem) : sizeof(TcwSmem)) + 128;
     const int grid = narrow ? (int)((c.N + TC_MEM - 1) / TC_MEM) : (int)((c.N + TCW_M - 1) / TCW_M);
@@ -69,14 +69,13 @@ int mlp_reverse_launch(Handle* h, const void* dLdu, void* du0, void* dp) {
     memset(&a, 0, sizeof(a));
     a.p = (const T*)h->cur_p; a.ckpt = (T*)h->d_ckpt; a.save_of_step = h->d_save_of_step; a.dLdu = (const T*)dLdu;
     a.du0 = (T*)du0; a.partials = (T*)h->d_partials; a.dp = (T*)dp; a.N = c.N; a.S = h->S; a.tb = h->tb;
-    for (int j = 0; j < 4; j++) { a.cost_a[j] = h->cost_av[j]; a.cost_b[j] = h->cost_bv[j]; } a.flags = (c.flags & B200ADJ_FLAG_NO_START) ? 1u : 0u;
+    for (int j = 0; j < 4; j++) { a.cost_a[j] = h->cost_av[j]; a.cost_b[j] = h->cost_bv[j]; } a.flags = kernel_flags(h) & KF_NO_START;
     const size_t smem = sizeof(MlpSmem<T>);
-    a.Npad = h->Npad;
     if (h->nev > 0) { a.event_of_step = h->d_event_of_step; a.ev_s = h->d_ev_s; a.ev_c = h->d_ev_c; }
-#define B200_MLP_REV(COSTV, TAPEV)                                                                                          \
+#define B200_MLP_REV(COSTV, GAUSSV)                                                                                         \
     do {                                                                                                                    \
-        if (cudaFuncSetAttribute(mlp_reverse_kernel<T, COSTV, TAPEV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return B200ADJ_ERR_CUDA; \
-        mlp_reverse_kernel<T, COSTV, TAPEV><<<h->grid, MLP_THREADS, smem, h->stream>>>(a);                                  \
+        if (cudaFuncSetAttribute(mlp_reverse_kernel<T, COSTV, GAUSSV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return B200ADJ_ERR_CUDA; \
+        mlp_reverse_kernel<T, COSTV, GAUSSV><<<h->grid, MLP_THREADS, smem, h->stream>>>(a);                                 \
     } while (0)
     const bool ex = c.cost_kind == B200ADJ_COST_EXPLICIT;
     if (c.sensealg == B200ADJ_SA_GAUSS) { if (ex) B200_MLP_REV(COST_EXPLICIT, true); else B200_MLP_REV(COST_AFFINE, true); }
@@ -90,12 +89,12 @@ int mlp_reverse_launch(Handle* h, const void* dLdu, void* du0, void* dp) {
 
 int mlp_forward_dispatch(Handle* h, const void* u0, const void* p, void* saved, int32_t* status) {
     const b200adj_cfg& c = h->cfg;
-    return h->mlp_tc ? mlp_tc_forward_launch(h, u0, p, saved, status)
+    return is_mlp_tc(h) ? mlp_tc_forward_launch(h, u0, p, saved, status)
          : c.dtype != B200ADJ_F64 ? mlp_forward_launch<float>(h, u0, p, saved, status) : mlp_forward_launch<double>(h, u0, p, saved, status);
 }
 int mlp_reverse_dispatch(Handle* h, const void* dLdu, void* du0, void* dp) {
     const b200adj_cfg& c = h->cfg;
-    return h->mlp_tc ? mlp_tc_reverse_launch(h, dLdu, du0, dp)
+    return is_mlp_tc(h) ? mlp_tc_reverse_launch(h, dLdu, du0, dp)
          : c.dtype != B200ADJ_F64 ? mlp_reverse_launch<float>(h, dLdu, du0, dp) : mlp_reverse_launch<double>(h, dLdu, du0, dp);
 }
 }  // namespace b200adj

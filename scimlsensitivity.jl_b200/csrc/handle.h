@@ -24,8 +24,18 @@
 
 namespace b200adj {
 
+// Which kernel framework serves a handle; decided once by b200adj_create.
+enum class Path {
+    FIXED,      // fixed-step Tsit5 on the dt grid (ode_tsit5.cuh, tsit5_quad.cuh; F64, and F32 for LV / Lorenz)
+    T5A,        // per-member dense Tsit5 (tsit5_adaptive.cuh): adaptive, or fixed step with off-grid save times
+    ROS,        // Rosenbrock23 (ros23.cuh)
+    SDE,        // Euler-Maruyama / Euler-Heun (sde_em.cuh)
+    MLP         // neural ODE family (mlp.cuh; BF16_F32ACC: mlp_tc.cuh, mlp_tc_wide.cuh)
+};
+
 struct Handle {
     b200adj_cfg cfg;
+    Path path = Path::FIXED;
     std::vector<double> saveat;
     std::vector<int32_t> save_of_step;
     int S = 0;
@@ -38,14 +48,10 @@ struct Handle {
     double* d_noise = nullptr;        // [S][m][N] (SDE, stored-noise mode)
     double* d_partials = nullptr;     // [grid][P]
     double* d_adj_dense = nullptr;    // QuadratureAdjoint, fixed-step Tsit5: [S][8][d][Npad]
-    int64_t Ktot = 0;
-    size_t qpart_blocks_fixed = 0;
     unsigned long long* d_trace = nullptr;   // [grid][3] block trace (B200ADJ_FLAG_TRACE)
     unsigned int* d_ticket = nullptr;
     int32_t* d_save_of_step = nullptr;
-    // adaptive path: per-member dense forward / reverse solutions
-    bool fixed_dt = false;            // fixed-step Tsit5 routed to the dense per-member framework (off-grid save times)
-    bool adaptive = false; int maxs = 0; int nk = 2;     // nk: dense-output stages stored per step (Rosenbrock23 2, Tsit5 7)
+    int maxs = 0;                     // T5A / ROS: per-member step capacity of the dense forward / reverse solutions
     double adj_abstol = 0, adj_reltol = 0;   // <= 0: use the forward tolerances
     // named cost family, per component (b200adj_set_cost_family; the scalar entry points broadcast):
     //   discrete (COST_AFFINE)  dgdu = cost_av .* u + cost_bv,  dgdp = dgdp_c .* p + dgdp_e   at every save time
@@ -55,14 +61,13 @@ struct Handle {
     bool has_dgdp = false, has_cdgdp = false;
     double dgdp_c[8] = {0}, dgdp_e[8] = {0}, cdgdp_c[8] = {0}, cdgdp_e[8] = {0};
     float* d_kst = nullptr;           // tensor-core MLP path: the forward stages of every step ([S][7][2][N] floats)
-    bool mlp_tc = false;              // BF16_F32ACC: every GEMM-shaped piece of the time loop on wgmma (mlp_tc.cuh)
     double *r_ft = nullptr, *r_fu = nullptr, *r_fk = nullptr, *d_saveat = nullptr;
-    // QuadratureAdjoint on the adaptive steppers (allocated at the first Quadrature reverse pass): member-major reverse dense
-    // solution + member-major copy of the forward one (quadgk.cuh)
+    // QuadratureAdjoint on T5A / ROS (allocated at the first Quadrature reverse pass): member-major reverse dense solution +
+    // member-major copy of the forward one (quadgk.cuh)
     double *r_rrec = nullptr, *r_rend = nullptr, *r_ftT = nullptr, *r_frecT = nullptr;
     int32_t *r_fn = nullptr, *r_rn = nullptr;
     // quadgk scratch of the QuadratureAdjoint kernels, sized per RESIDENT warp of the persistent grid qgrid (quadgk.cuh)
-    double *r_qseg = nullptr, *r_qkey = nullptr; int maxseg = 0; int qgrid = 0; size_t qpartials_blocks = 0; int saveat_dev_K = 0;
+    double *r_qseg = nullptr, *r_qkey = nullptr; int maxseg = 0; int qgrid = 0; size_t qpartials_blocks = 0;
     // forward save table (the primal output of b200adj_forward) kept apart from the reverse pass' jump times
     int fwd_K = 0; std::vector<double> fwd_saveat; std::vector<int32_t> fwd_save_of_step; int32_t* d_fwd_save_of_step = nullptr; double* d_fwd_saveat = nullptr;
     // staging (buffers_on_device == 0)
@@ -102,6 +107,17 @@ struct Handle {
     } while (0)
 
 inline bool is_sde(const b200adj_cfg& c) { return c.stepper == B200ADJ_ST_EM || c.stepper == B200ADJ_ST_EULER_HEUN; }
+inline bool is_adaptive(const Handle* h) { return h->path == Path::T5A || h->path == Path::ROS; }
+// T5A run with a constant step and no error control (fixed-step Tsit5 with off-grid save times)
+inline bool is_fixed_dt(const Handle* h) { return h->path == Path::T5A && h->cfg.stepper == B200ADJ_ST_TSIT5_FIXED; }
+inline bool is_mlp_tc(const Handle* h) { return h->path == Path::MLP && h->cfg.dtype == B200ADJ_BF16_F32ACC; }
+// the kernels' `flags` word (KF_* bits, ode_tsit5.cuh)
+inline uint32_t kernel_flags(const Handle* h) {
+    const uint32_t f = h->cfg.flags;
+    return ((f & B200ADJ_FLAG_NO_START) ? KF_NO_START : 0u) | ((f & B200ADJ_FLAG_NO_CHECKPOINTING) ? KF_NO_CHECKPOINTING : 0u) |
+           ((f & B200ADJ_FLAG_CKPT_EVERY_STEP) ? KF_CKPT_EVERY_STEP : 0u) | (h->cont_on ? KF_CONT_COST : 0u) |
+           (is_fixed_dt(h) ? KF_FIXED_DT : 0u);
+}
 inline size_t esz(const b200adj_cfg& c) { return c.dtype == B200ADJ_F64 ? sizeof(double) : sizeof(float); }   // BF16_F32ACC: fp32 buffers at the ABI
 
 void tsit5_weights(double th, double* w, double (*Rout)[4] = nullptr);
@@ -131,10 +147,14 @@ struct FamilyVTable {
     int (*t5a_rev)(Handle*, const T5aArgs&);
     int (*ros_fwd)(Handle*, const RosArgs&);         // Rosenbrock23 (null when the family has no jac / djac / dvjp_p)
     int (*ros_rev)(Handle*, const RosArgs&);
+    int (*fwd_f32)(Handle*, const OdeFwdArgsT<float>&);     // fixed-step Tsit5 in F32 (built-in LV / Lorenz; null elsewhere)
+    int (*rev_f32)(Handle*, const OdeRevArgsT<float>&);
 };
-constexpr uint32_t B200ADJ_PLUGIN_ABI = 0x00020000u ^ (uint32_t)sizeof(Handle) ^ ((uint32_t)sizeof(OdeRevArgs) << 8) ^ ((uint32_t)sizeof(T5aArgs) << 16);
+constexpr uint32_t B200ADJ_PLUGIN_ABI = 0x00020000u ^ (uint32_t)sizeof(Handle) ^ ((uint32_t)sizeof(OdeRevArgs) << 8) ^
+                                        ((uint32_t)sizeof(T5aArgs) << 16) ^ ((uint32_t)sizeof(FamilyVTable) << 24);
 constexpr int B200ADJ_FAM_USER_BASE_ID = 100;
-const FamilyVTable* family_lookup(int id);          // api.cu: registered plug-in families
+// api.cu: the ODE families, built-in (id < B200ADJ_FAM_USER_BASE_ID) and registered plug-ins; null for the SDE / MLP families
+const FamilyVTable* family_lookup(int id);
 
 // ---- dispatch entry points, one explicit instantiation per family in disp_*.cu ----
 template <class Fam> int launch_fwd(Handle* h, const OdeFwdArgs& a);
@@ -164,7 +184,7 @@ template <class K> inline int quad_launch_grid(const Handle* h, K kernel, size_t
     const int cap = nb * h->nsm;
     return h->qgrid < cap ? h->qgrid : cap;
 }
-int ensure_quad_buffers(Handle* h);      // api.cu: lazily allocates the buffers above and the quadgk scratch
+int ensure_quad_buffers(Handle* h);      // api.cu: lazily allocates QuadratureAdjoint's dense solutions and the quadgk scratch
 inline size_t quad_smem(int maxseg) { return (size_t)QUAD_WARPS * (QUAD_SKEYS + (maxseg >> 5)) * sizeof(double); }
 inline size_t quad_seg_doubles(int P, int maxseg, int qgrid) { return (size_t)qgrid * QUAD_WARPS * maxseg * (size_t)(((P + 4 + 3) / 4) * 4); }
 

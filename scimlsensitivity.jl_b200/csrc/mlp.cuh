@@ -29,8 +29,7 @@ template <class T> struct MlpArgs {
     const T* u0; const T* p; T* ckpt; T* saved; const int32_t* save_of_step; int32_t* status;
     const T* dLdu; T* du0; T* partials; T* dp;     // partials [grid][P]
     int64_t N; int32_t S; double cost_a[4], cost_b[4]; uint32_t flags;
-    void* tapeA; void* tapeB; int64_t Ktot, Npad;     // (superseded bf16 tape formulation: unused)
-    float* kst;                                       // tensor-core path: forward stages k1..k7 per step, [S][7][2][N] (or null: recompute)
+    float* kst;                                       // tensor-core path: forward stages k1..k7 per step, [S][7][2][N]
     Tsit5Tables tb;
     // hybrid neural ODE (test/Core5/HybridNODE.jl:20-24, PresetTimeCallback on a neural RHS): preset-time events on the dt grid,
     // event_of_step[n] = e when u <- ev_s[e] .* u + ev_c[e] fires at t_n (else -1); null = none.  CUDA-core kernels (F64 / F32).
@@ -136,25 +135,10 @@ template <class T> struct MlpGrad {
 };
 
 // grad += c * F(y)' L  with the activations of the last forward/backward pair (s.y, s.L, s.H1, s.H2, s.D1, s.D2), members >= nvalid masked
-template <class T, bool TAPE>
-__device__ __forceinline__ void mlp_accumulate(const MlpSmem<T>& s, MlpGrad<T>& g, T c, int nvalid,
-                                               __nv_bfloat16* tapeA, __nv_bfloat16* tapeB, int64_t Ktot, int64_t kbase) {
+template <class T>
+__device__ __forceinline__ void mlp_accumulate(const MlpSmem<T>& s, MlpGrad<T>& g, T c, int nvalid) {
     const int i0 = (threadIdx.x / 16) * 4, j0 = (threadIdx.x % 16) * 4, t = threadIdx.x;
-    if (TAPE) {
-        // dW2 goes to the tensor cores: write this point's operands (c * Delta2 and H1, 64 rows x 32 members each) as
-        // K-major bf16; thread -> (row, 8-member segment) -> one 16 B store per tape; members past nvalid contribute 0
-        const int row = t >> 2, seg = (t & 3) * 8;
-        __align__(16) __nv_bfloat16 va[8], vb[8];
-#pragma unroll
-        for (int q = 0; q < 8; q++) {
-            const bool ok = seg + q < nvalid;
-            va[q] = __float2bfloat16(ok ? (float)(c * s.D2[row][seg + q]) : 0.f);
-            vb[q] = __float2bfloat16(ok ? (float)s.H1[row][seg + q] : 0.f);
-        }
-        *reinterpret_cast<uint4*>(tapeA + (int64_t)row * Ktot + kbase + seg) = *reinterpret_cast<const uint4*>(va);
-        *reinterpret_cast<uint4*>(tapeB + (int64_t)row * Ktot + kbase + seg) = *reinterpret_cast<const uint4*>(vb);
-    }
-    for (int b = 0; b < (TAPE ? 0 : nvalid); b++) {
+    for (int b = 0; b < nvalid; b++) {
         T d[4], h[4];
 #pragma unroll
         for (int r = 0; r < 4; r++) { d[r] = c * s.D2[i0 + r][b]; h[r] = s.H1[j0 + r][b]; }
@@ -246,7 +230,6 @@ __global__ void __launch_bounds__(MLP_THREADS) mlp_forward_kernel(const __grid_c
 // output and y_g from the forward dense output (src/gauss_adjoint.jl:745-759) ----
 template <class T, int COST, bool GAUSS>
 __global__ void __launch_bounds__(MLP_THREADS) mlp_reverse_kernel(const __grid_constant__ MlpArgs<T> a) {
-    constexpr bool TAPE = false;
     extern __shared__ __align__(16) unsigned char smem_raw[];
     MlpSmem<T>& s = *reinterpret_cast<MlpSmem<T>*>(smem_raw);
     const int64_t N = a.N, base = (int64_t)blockIdx.x * MLP_TB;
@@ -326,8 +309,7 @@ __global__ void __launch_bounds__(MLP_THREADS) mlp_reverse_kernel(const __grid_c
             mlp_forward<T>(s);
             mlp_backward<T>(s);
             if (own) s.ka[st][c][b] = s.JTL[c][b];
-            if (!GAUSS) mlp_accumulate<T, TAPE>(s, g, (T)tb.hA[6][st], nvalid, (__nv_bfloat16*)a.tapeA, (__nv_bfloat16*)a.tapeB, a.Ktot,
-                                                ((int64_t)(a.S - 1 - n) * 6 + st) * a.Npad + base);
+            if (!GAUSS) mlp_accumulate<T>(s, g, (T)tb.hA[6][st], nvalid);
             __syncthreads();
         }
         if (GAUSS) {
@@ -341,7 +323,7 @@ __global__ void __launch_bounds__(MLP_THREADS) mlp_reverse_kernel(const __grid_c
                 __syncthreads();
                 mlp_forward<T>(s);
                 mlp_backward<T>(s);
-                mlp_accumulate<T, TAPE>(s, g, (T)tb.hGW[gq], nvalid, nullptr, nullptr, 0, 0);
+                mlp_accumulate<T>(s, g, (T)tb.hGW[gq], nvalid);
                 __syncthreads();
             }
         }
@@ -351,7 +333,7 @@ __global__ void __launch_bounds__(MLP_THREADS) mlp_reverse_kernel(const __grid_c
             for (int j = 0; j < 6; j++) l = fma(tb.hA[6][j], (double)s.ka[j][c][b], l);
             s.lam[c][b] = (T)l;
         }
-        { const int ks = a.save_of_step[n]; if (ks >= 0 && !((a.flags & 1u) && n == 0)) cotangent(ks, s.ulo); }
+        { const int ks = a.save_of_step[n]; if (ks >= 0 && !((a.flags & KF_NO_START) && n == 0)) cotangent(ks, s.ulo); }
         if (own) { s.uhi[c][b] = s.ulo[c][b]; s.kf[6][c][b] = s.kf[0][c][b]; }
         if (a.event_of_step) {
             // reverse affect of u+ = s .* u- + c at t_n, after the loss jump of the same time: lam- = s .* lam+

@@ -273,7 +273,7 @@ __global__ void __launch_bounds__(TCW_M) mlp_tcw_reverse_kernel(const __grid_con
             for (int j = 0; j < 6; j++) l = fma(tb.hA[6][j], (double)ka[j][c], l);
             lam[c] = (float)l;
         }
-        { const int ks = a.save_of_step[n]; if (ks >= 0 && !((a.flags & 1u) && n == 0)) cotangent(ks, ulo); }
+        { const int ks = a.save_of_step[n]; if (ks >= 0 && !((a.flags & KF_NO_START) && n == 0)) cotangent(ks, ulo); }
         uhi[0] = ulo[0]; uhi[1] = ulo[1];
     }
     if (live) { a.du0[col] = lam[0]; a.du0[N + col] = lam[1]; }

@@ -72,6 +72,13 @@ template <class R> struct OdeFwdArgsT {
 };
 using OdeFwdArgs = OdeFwdArgsT<double>;
 
+// bits of the kernels' `flags` word (OdeRevArgsT, T5aArgs, RosArgs, SdeRevArgs, MlpArgs); handle.h::kernel_flags builds it
+constexpr uint32_t KF_NO_START = 1u;            // no loss jump at t0 (B200ADJ_FLAG_NO_START)
+constexpr uint32_t KF_NO_CHECKPOINTING = 2u;    // BacksolveAdjoint(checkpointing = false)
+constexpr uint32_t KF_CKPT_EVERY_STEP = 4u;     // Backsolve: checkpoints at every step instead of the save times
+constexpr uint32_t KF_CONT_COST = 8u;           // continuous cost: dlam -= dgdu_continuous(y)
+constexpr uint32_t KF_FIXED_DT = 16u;           // T5A kernels: constant step dt0, no error control
+
 template <class R> struct OdeRevArgsT {
     const R* ckpt;      // [S+1][D][N]
     const R* p;         // [P] or [P][N]
@@ -88,8 +95,8 @@ template <class R> struct OdeRevArgsT {
     int32_t slots;           // member slots per block (= checkpoint tile width); blockDim.x > slots => the top warp row rotates
     int32_t ckpt_every;      // C > 1 (SEG kernels): forward states kept every C steps, each segment re-solved into shared memory
     R cost_a[4], cost_b[4];   // COST_AFFINE, per component: dgdu_discrete = cost_a .* u(t_k) + cost_b
-    R cont_a[4], cont_b[4];   // continuous cost g = sum_j cont_a_j/2 u_j^2 + cont_b_j u_j:  dlam -= dgdu_continuous(y)  (flags bit3)
-    uint32_t flags;          // bit0 no_start, bit1 no checkpointing (backsolve), bit2 ckpt every step, bit3 continuous cost
+    R cont_a[4], cont_b[4];   // continuous cost g = sum_j cont_a_j/2 u_j^2 + cont_b_j u_j:  dlam -= dgdu_continuous(y)  (KF_CONT_COST)
+    uint32_t flags;          // KF_* bits
     R* adj_dense;       // SA_QUAD: [S][8][D][Npad] = (lambda at the start of reverse step n, ka'[0..6]) per step
     unsigned long long* trace;   // optional [gridDim][3] = (smid, globaltimer at block start, at block end) or null
     const int32_t* event_of_step; const double* ev_s; const double* ev_c; const double* ev_ps; const double* ev_pc; int32_t nev;   // EV kernels
@@ -438,7 +445,7 @@ __global__ void __maxnreg__(B200_REV_MAXREG) tsit5_reverse_kernel(const __grid_c
         load_state<D>(a.ckpt + (int64_t)a.S * cstride, Npad, gi, y);
         { int ks = a.save_of_step[a.S]; if (ks >= 0) add_cotangent<D, COST>(a, ks, stride, N, i, y, lam); }
         R ky[7][D], kl[7][D], ys[D], ls[D], dg[P];
-        const bool ckpt_on = !(a.flags & 2u), every = (a.flags & 4u);
+        const bool ckpt_on = !(a.flags & KF_NO_CHECKPOINTING), every = (a.flags & KF_CKPT_EVERY_STEP);
         bool fsal = false;
         for (int n = a.S - 1; n >= 0; n--) {
             if (!fsal) {
@@ -718,7 +725,7 @@ __global__ void __maxnreg__(B200_REV_MAXREG) tsit5_reverse_kernel(const __grid_c
 
             // ---- jump at t_n (ReverseLossCallback): lam += dgdu(t_k), FSAL invalidated => recompute ka[0] ----
             const int ks = a.save_of_step[n];
-            if (ks >= 0 && !((a.flags & 1u) && n == 0)) {
+            if (ks >= 0 && !((a.flags & KF_NO_START) && n == 0)) {
                 add_cotangent<D, COST>(a, ks, stride, N, member_i(), ulo, lam);
                 Fam::vjp_u(ulo, p, lam, ka[0]);
                 add_continuous<D, CONT>(a, ulo, ka[0]);

@@ -40,7 +40,7 @@ struct RosArgs {
     double* qseg; double* qkey; int32_t maxseg;                  // quadgk scratch per resident warp: segments [maxseg][SEGW], keys [maxseg] (quadgk.cuh)
     int64_t N; int32_t K; int32_t maxs;
     double t0, t1, abstol, reltol, quad_abstol, quad_reltol, cost_a[4], cost_b[4];
-    uint32_t flags;                                               // bit0 no_start
+    uint32_t flags;                                               // KF_* bits
 };
 
 __device__ constexpr double ROS_D = 0.29289321881345247559915563789515;
@@ -282,7 +282,7 @@ __global__ void __launch_bounds__(256) ros23_reverse_kernel(RosArgs a) {
     bool fsal_ok = false, overflow = false;
     auto jump_if_at = [&](double tt) {
         while (cur >= 0 && fabs(a.saveat[cur] - tt) <= EPS100 * fmax(fabs(tt), 1.0)) {
-            if (!((a.flags & 1u) && cur == 0)) {
+            if (!((a.flags & KF_NO_START) && cur == 0)) {
                 double y[D];
                 if (COST == COST_EXPLICIT) {
 #pragma unroll
@@ -476,7 +476,7 @@ __global__ void __launch_bounds__(256) ros23_aug_reverse_kernel(RosArgs a) {
     double t = T;
     int cur = a.K - 1, ck = sol.n;
     bool fsal_ok = false, failed = false;
-    const bool ckpt_on = !(a.flags & 2u), every = (a.flags & 4u);
+    const bool ckpt_on = !(a.flags & KF_NO_CHECKPOINTING), every = (a.flags & KF_CKPT_EVERY_STEP);
     if (SA == SA_BACKSOLVE) {
 #pragma unroll
         for (int j = 0; j < D; j++) z[YO + j] = a.fu[((int64_t)sol.n * D + j) * N + i];     // y(T) = sol.u[end]
@@ -501,7 +501,7 @@ __global__ void __launch_bounds__(256) ros23_aug_reverse_kernel(RosArgs a) {
     };
     auto jump_if_at = [&](double tt) {
         while (cur >= 0 && fabs(a.saveat[cur] - tt) <= EPS100 * fmax(fabs(tt), 1.0)) {
-            if (!((a.flags & 1u) && cur == 0 && SA != SA_BACKSOLVE)) {
+            if (!((a.flags & KF_NO_START) && cur == 0 && SA != SA_BACKSOLVE)) {
                 if (COST == COST_EXPLICIT) {
 #pragma unroll
                     for (int j = 0; j < D; j++) z[j] += a.dLdu[((int64_t)cur * D + j) * N + i];

@@ -163,14 +163,14 @@ __global__ void __launch_bounds__(512) sde_backsolve_kernel(SdeRevArgs a) {
 #pragma unroll
     for (int q = 0; q < P; q++) mu[q] = 0.0;
     load_state<D>(a.ckpt + (int64_t)a.S * stride, N, i, y);
-    const bool ckpt_on = !(a.flags & 2u), every = (a.flags & 4u);
+    const bool ckpt_on = !(a.flags & KF_NO_CHECKPOINTING), every = (a.flags & KF_CKPT_EVERY_STEP);
     const double h = a.h, sq = sqrt(a.h);
     for (int n = a.S; n >= 0; n--) {
         // callbacks at grid point n: checkpoint reset, then the loss jump
         const int ks = a.save_of_step[n];
         if (INTERP || (ckpt_on && (every || ks >= 0))) load_state<D>(a.ckpt + (int64_t)n * stride, N, i, y);
         // no_start skips the jump of the first save time for every sensealg but Backsolve (src/adjoint_common.jl:761)
-        if (ks >= 0 && !(INTERP && (a.flags & 1u) && ks == 0)) {
+        if (ks >= 0 && !(INTERP && (a.flags & KF_NO_START) && ks == 0)) {
             if (COST == COST_EXPLICIT) {
 #pragma unroll
                 for (int j = 0; j < D; j++) lam[j] += __ldg(a.dLdu + (int64_t)ks * stride + (int64_t)j * N + i);

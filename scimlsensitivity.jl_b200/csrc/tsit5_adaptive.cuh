@@ -33,7 +33,7 @@ struct T5aArgs {
     // preset-time events u <- scale .* u + shift (the hybrid-system adjoint of src/callback_tracking.jl:232-480 for the
     // affine affect family, save_positions = (false, false)): same events for every member, times ascending in (t0, t1)
     int32_t nev; const double* ev_t; const double* ev_s; const double* ev_c;      // [E], [E][D], [E][D]
-    double cont_a[4], cont_b[4];  // flags bit3: continuous cost g(u) = cont_a/2 |u|^2 + cont_b sum(u), dlam -= dgdu_continuous(y) (accumulate_cost!)
+    double cont_a[4], cont_b[4];  // KF_CONT_COST: continuous cost g(u) = cont_a/2 |u|^2 + cont_b sum(u), dlam -= dgdu_continuous(y) (accumulate_cost!)
     const double* ev_ps; const double* ev_pc;     // [E][P] or null: parameter-changing affect p <- ps .* p + pc (reset_p of the reference)
     // [E] or null: affect that adds a parameter to a state, u[ev_ac[e]] += ev_af[e] * p[ev_ak[e]] with the parameters in force before
     // the event ("Dosing example", test/Callbacks1/discrete_callbacks.jl:401-427: integrator.u[1] += integrator.p[2]); ev_ac[e] < 0: none
@@ -252,7 +252,7 @@ __global__ void __launch_bounds__(256) t5a_forward_kernel(const __grid_constant_
         ksave++;
     }
     int ev = 0;                                   // next event ahead of t (event times are tstops of the forward solve)
-    const bool fixed = (a.flags & 16u) != 0;      // constant step dt0, no error control (fixed-step Tsit5 with off-grid save times)
+    const bool fixed = (a.flags & KF_FIXED_DT) != 0;      // constant step dt0, no error control (fixed-step Tsit5 with off-grid save times)
     bool after_event = false;                     // CC: the step starts on an event (condition ~0 with a random sign)
     int nfound = 0;
     const double cc_lev = CC ? t5_cc_level<P>(a, p) : 0.0;
@@ -471,7 +471,7 @@ __global__ void __launch_bounds__(256) t5a_reverse_kernel(const __grid_constant_
         Fam::vjp_u(y, p, x, dx);
 #pragma unroll
         for (int j = 0; j < D; j++) dx[j] = -dx[j];
-        if (a.flags & 8u) {                                          // src/derivative_wrappers.jl:1411-1442
+        if (a.flags & KF_CONT_COST) {                                          // src/derivative_wrappers.jl:1411-1442
 #pragma unroll
             for (int j = 0; j < D; j++) dx[j] -= a.cont_a[j] * y[j] + a.cont_b[j];
         }
@@ -489,7 +489,7 @@ __global__ void __launch_bounds__(256) t5a_reverse_kernel(const __grid_constant_
     auto evt = [&](int e) { return CC ? a.cc_t[(int64_t)e * N + i] : a.ev_t[e]; };
     int cur = a.K - 1, nrev = 0, ck = sol.n, evc = (CC ? a.cc_n[i] : a.nev) - 1;
     bool fsal_ok = false, overflow = false;
-    const bool ckpt_on = !(a.flags & 2u), every = (a.flags & 4u);
+    const bool ckpt_on = !(a.flags & KF_NO_CHECKPOINTING), every = (a.flags & KF_CKPT_EVERY_STEP);
     if (SA == SA_BACKSOLVE) {
 #pragma unroll
         for (int j = 0; j < D; j++) z[YO + j] = sol.record(sol.n)[j];     // y(T) = sol.u[end]
@@ -597,7 +597,7 @@ __global__ void __launch_bounds__(256) t5a_reverse_kernel(const __grid_constant_
     };
     auto jump_if_at = [&](double tt) {
         while (cur >= 0 && fabs(a.saveat[cur] - tt) <= EPS100 * fmax(fabs(tt), 1.0)) {
-            if (!((a.flags & 1u) && cur == 0 && SA != SA_BACKSOLVE)) {
+            if (!((a.flags & KF_NO_START) && cur == 0 && SA != SA_BACKSOLVE)) {
                 if (COST == COST_EXPLICIT) {
 #pragma unroll
                     for (int j = 0; j < D; j++) z[j] += a.dLdu[((int64_t)cur * D + j) * N + i];
@@ -618,7 +618,7 @@ __global__ void __launch_bounds__(256) t5a_reverse_kernel(const __grid_constant_
     ckpt_if_at(t);
     jump_if_at(t);
     double h = a.dt0 > 0 ? -a.dt0 : -1e-4 * (T - t0), qold = 1e-4;
-    const bool fixed = (a.flags & 16u) != 0;
+    const bool fixed = (a.flags & KF_FIXED_DT) != 0;
     long iters = 0;
     while (t > t0 && sol.n > 0) {
         if (++iters > 50000000L || (SA == SA_QUAD && nrev >= a.maxs)) { overflow = true; break; }
