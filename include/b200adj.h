@@ -215,6 +215,25 @@ int32_t b200adj_set_continuous_callback_params(void* handle, int32_t lparam, dou
 /* event lists found by the last forward pass: counts[N] (host, may be NULL), times[max_events][N] (host, may be NULL) */
 int32_t b200adj_event_times(void* handle, int32_t* counts, double* times);
 
+/* Number of conditions compiled into a family (its plug-in was built with B200ADJ_FAMILY_HAS_EVENTS, csrc/family_plugin.inc):
+ * the `len` of VectorContinuousCallback(condition, affect!, len).  0 for every built-in family and for plug-ins without events. */
+int32_t b200adj_family_conditions(int32_t family, int32_t* nc);
+/* VectorContinuousCallback of the reference (the callback type of test/Callbacks2/vector_continuous_callbacks.jl; reverse-pass
+ * treatment of src/callback_tracking.jl:232-480) with the condition(out, u, t, integrator) and affect!(integrator, ev) compiled
+ * into the family struct, save_positions = (false, false).  A mode of the continuous callback above: each member finds its own
+ * events (all nc conditions are sampled on the dense output of every accepted step, the first crossing interval is bisected to
+ * the last bit, conditions whose roots have the same bits fire together), b200adj_event_times reports them and
+ * b200adj_event_flags which conditions fired.  The reverse pass applies, with c = the lowest condition that fired,
+ *   lam- = mu_u - dg_c/du (w / den),  dG/dp += mu_p - dg_c/dp (w / den),  den = dg_c/du . f(u-) + dg_c/dt,
+ *   w = mu_u . f(u-) - lam+ . f(u+),  (mu_u, mu_p) = the affect's VJP with lam+.
+ * direction[nc]: -1 downwards only, +1 upwards only, 0 both.  Adaptive Tsit5, Interpolating / Gauss / GaussKronrod / Backsolve;
+ * not together with b200adj_set_events; nc must be the family's.  enabled = 0 removes the callback (either mode).  Call before
+ * b200adj_forward. */
+int32_t b200adj_set_family_events(void* handle, int32_t enabled, int32_t nc, const int32_t* direction, int32_t max_events);
+/* event words of the last forward pass with family events: ev[max_events][N] (host); the word of event e of member i has bit 2c
+ * set when condition c fired and bit 2c + 1 when it crossed upwards.  Entries past the member's event count are undefined. */
+int32_t b200adj_event_flags(void* handle, int32_t* ev);
+
 /* SDE helper for parity tests: copy out the Wiener increments the forward pass used, dW[S][m][N]. */
 int32_t b200adj_get_noise(void* handle, void* dW_out);
 

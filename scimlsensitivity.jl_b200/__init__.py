@@ -12,7 +12,7 @@ from .concrete_solve import (ChainRulesOriginator, NoTangent, ReverseDiffOrigina
 from .distributed import allreduce_dp, shard_bounds
 from .engine import DeviceEnsemble
 from .family_plugin import build_family_plugin, register_family
-from .problems import (EM, AdjointSensitivityParameterCompatibilityError, AffineAffect, AffineCost, ContinuousCallback, PresetTimeCallback, EnsembleB200, EnsembleProblem,
+from .problems import (EM, AdjointSensitivityParameterCompatibilityError, AffineAffect, AffineCost, ContinuousCallback, VectorContinuousCallback, PresetTimeCallback, EnsembleB200, EnsembleProblem,
                        EnsembleSolution, EulerHeun, FAMILIES, ODEProblem, ParamAffine, QuadraticRunningCost, Rosenbrock23, SDEProblem, Tsit5)
 from .sensitivity_algorithms import (B200Adjoint, B200VJP, BacksolveAdjoint, EnzymeVJP, GaussAdjoint, GaussKronrodAdjoint,
                                      InterpolatingAdjoint, MooncakeVJP, QuadratureAdjoint, ReactantVJP,

@@ -21,7 +21,7 @@ COST = {"explicit": 0, "affine": 1}
 FLAG_NO_START, FLAG_NO_CHECKPOINTING, FLAG_CKPT_EVERY_STEP, FLAG_STORED_NOISE, FLAG_TRACE, FLAG_NO_ROTATE, FLAG_DENSE_FORWARD, FLAG_NCCL_ALLREDUCE = 1, 2, 4, 8, 16, 32, 64, 128
 ERR = {0: "OK", -1: "INVALID", -2: "UNSUPPORTED", -3: "NO_DEVICE", -4: "CUDA", -5: "STATE", -6: "OOM"}
 
-EXPORTS = ["b200adj_create", "b200adj_forward", "b200adj_reverse", "b200adj_set_reverse_options", "b200adj_set_tolerances", "b200adj_set_continuous_cost", "b200adj_set_cost_family", "b200adj_register_family", "b200adj_family_info", "b200adj_set_events", "b200adj_set_event_param_shift", "b200adj_set_continuous_callback", "b200adj_set_continuous_callback_params", "b200adj_event_times", "b200adj_get_noise", "b200adj_set_stream",
+EXPORTS = ["b200adj_create", "b200adj_forward", "b200adj_reverse", "b200adj_set_reverse_options", "b200adj_set_tolerances", "b200adj_set_continuous_cost", "b200adj_set_cost_family", "b200adj_register_family", "b200adj_family_info", "b200adj_set_events", "b200adj_set_event_param_shift", "b200adj_set_continuous_callback", "b200adj_set_continuous_callback_params", "b200adj_event_times", "b200adj_family_conditions", "b200adj_set_family_events", "b200adj_event_flags", "b200adj_get_noise", "b200adj_set_stream",
            "b200adj_synchronize", "b200adj_launch_count", "b200adj_get_step_counts", "b200adj_get_block_trace", "b200adj_destroy",
            "b200adj_last_error", "b200adj_version", "b200adj_sizeof_cfg",
            "b200adj_comm_unique_id", "b200adj_comm_init", "b200adj_comm_init_all", "b200adj_comm_allreduce", "b200adj_comm_size", "b200adj_comm_is_fused"]
@@ -150,6 +150,12 @@ def load():
         lib.b200adj_set_continuous_callback_params.restype = C.c_int32
         lib.b200adj_event_times.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
         lib.b200adj_event_times.restype = C.c_int32
+        lib.b200adj_family_conditions.argtypes = [C.c_int32, C.POINTER(C.c_int32)]
+        lib.b200adj_family_conditions.restype = C.c_int32
+        lib.b200adj_set_family_events.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32]
+        lib.b200adj_set_family_events.restype = C.c_int32
+        lib.b200adj_event_flags.argtypes = [C.c_void_p, C.c_void_p]
+        lib.b200adj_event_flags.restype = C.c_int32
         lib.b200adj_get_noise.argtypes = [C.c_void_p, C.c_void_p]
         lib.b200adj_get_noise.restype = C.c_int32
         lib.b200adj_set_stream.argtypes = [C.c_void_p, C.c_void_p]
@@ -195,6 +201,15 @@ def _addr(x):
     if hasattr(x, "data_ptr"):
         return x.data_ptr()
     return x.ctypes.data
+
+
+def family_conditions(family_id):
+    """Number of conditions compiled into a family (0: none)."""
+    nc = C.c_int32()
+    rc = load().b200adj_family_conditions(int(family_id), C.byref(nc))
+    if rc != 0:
+        raise B200AdjError(rc, f"unknown family id {family_id}")
+    return nc.value
 
 
 def comm_unique_id():
@@ -312,6 +327,20 @@ class Handle:
         times = np.zeros((max_events, N), dtype=np.float64)
         self._check(self._lib.b200adj_event_times(self._h, counts.ctypes.data, times.ctypes.data))
         return counts, times
+
+    def set_family_events(self, nc, direction, max_events=64, enabled=True):
+        """State-dependent event with the conditions and affect compiled into the family; direction[nc] in {-1, 0, 1}."""
+        import numpy as np
+        dr = np.ascontiguousarray(direction, dtype=np.int32).reshape(-1)
+        self._check(self._lib.b200adj_set_family_events(self._h, 1 if enabled else 0, int(nc), dr.ctypes.data if len(dr) else None,
+                                                        int(max_events)))
+
+    def event_flags(self, N, max_events):
+        """-> words[max_events, N] (int32) of the last forward pass: bit 2c = condition c fired, bit 2c + 1 = upwards."""
+        import numpy as np
+        ev = np.zeros((max_events, N), dtype=np.int32)
+        self._check(self._lib.b200adj_event_flags(self._h, ev.ctypes.data))
+        return ev
 
     def step_counts(self, fwd, rev):
         self._check(self._lib.b200adj_get_step_counts(self._h, _addr(fwd), _addr(rev)))

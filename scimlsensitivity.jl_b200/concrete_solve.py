@@ -11,7 +11,7 @@ import numpy as np
 
 from . import distributed
 from .engine import DeviceEnsemble, _is_torch
-from .problems import (EM, AffineCost, ContinuousCallback, PresetTimeCallback, EnsembleB200, EnsembleProblem, EnsembleSolution, EulerHeun, FAMILIES, ODEProblem,
+from .problems import (EM, AffineCost, ContinuousCallback, VectorContinuousCallback, PresetTimeCallback, EnsembleB200, EnsembleProblem, EnsembleSolution, EulerHeun, FAMILIES, ODEProblem,
                        Rosenbrock23, SDEProblem, Tsit5, saveat_to_times)
 from .sensitivity_algorithms import (B200Adjoint, BacksolveAdjoint, GaussAdjoint, GaussKronrodAdjoint, InterpolatingAdjoint,
                                      QuadratureAdjoint, sensealg_name)
@@ -89,12 +89,14 @@ def solve(eprob, alg, ensemblealg=None, *, trajectories=None, saveat=None, sense
     prob = eprob.prob
     callback = kwargs.pop("callback", None) or prob.callback
     ccb = None
-    if isinstance(callback, ContinuousCallback):
-        # state-dependent event of the named condition / affect family: adaptive Tsit5, every member finds its own event times
+    if isinstance(callback, (ContinuousCallback, VectorContinuousCallback)):
+        # state-dependent event -- the named condition / affect family, or the conditions and affect compiled into the problem's
+        # family: adaptive Tsit5, every member finds its own event times
+        kind = type(callback).__name__
         if tuple(callback.save_positions) != (False, False):
-            raise NotImplementedError("ContinuousCallback: save_positions = (false, false) only")
+            raise NotImplementedError(f"{kind}: save_positions = (false, false) only")
         if not (isinstance(alg, Tsit5) and alg.code == "tsit5_adaptive"):
-            raise NotImplementedError("ContinuousCallback: built for the adaptive Tsit5 stepper")
+            raise NotImplementedError(f"{kind}: built for the adaptive Tsit5 stepper")
         ccb, callback = callback, None
     if callback is not None:
         # preset-time affine affects on the Tsit5 steppers

@@ -240,6 +240,8 @@ T5aArgs t5a_args(Handle* h) {
         for (int j = 0; j < 4; j++) { a.cc_scale[j] = h->cc_scale[j]; a.cc_shift[j] = h->cc_shift[j]; }
         a.cc_lparam = h->cc_lparam; a.cc_lcoef = h->cc_lcoef; a.cc_acomp = h->cc_acomp; a.cc_aparam = h->cc_aparam; a.cc_acoef = h->cc_acoef;
         a.cc_qcomp = h->cc_qcomp; a.cc_qcoef = h->cc_qcoef;
+        a.fe_nc = h->fe_nc; a.cc_ev = h->d_cc_ev;
+        for (int c = 0; c < 8; c++) a.fe_dir[c] = h->fe_dir[c];
     }
     return a;
 }
@@ -252,9 +254,27 @@ void free_all(Handle* h) {
     cudaFree(h->d_saveat); cudaFree(h->r_fn); cudaFree(h->r_rn); cudaFree(h->r_qseg); cudaFree(h->r_qkey);
     cudaFree(h->d_kst); cudaFree(h->d_adj_dense); cudaFree(h->d_trace); cudaFree(h->d_ckpt); cudaFree(h->d_noise); cudaFree(h->d_partials); cudaFree(h->d_ticket); cudaFree(h->d_save_of_step); cudaFree(h->d_fwd_save_of_step); cudaFree(h->d_fwd_saveat);
     cudaFree(h->s_u0); cudaFree(h->s_p); cudaFree(h->s_saved); cudaFree(h->s_dLdu); cudaFree(h->s_du0); cudaFree(h->s_dp); cudaFree(h->s_dW);
-    cudaFree(h->d_cc_t); cudaFree(h->d_cc_n);
+    cudaFree(h->d_cc_t); cudaFree(h->d_cc_n); cudaFree(h->d_cc_ev);
     cudaFree(h->s_status); cudaFree(h->d_event_of_step); cudaFree(h->d_ev_ac); cudaFree(h->d_ev_ak); cudaFree(h->d_ev_af); cudaFree(h->d_ev_t); cudaFree(h->d_ev_s); cudaFree(h->d_ev_c); cudaFree(h->d_ev_ps); cudaFree(h->d_ev_pc);
     if (h->own_stream) cudaStreamDestroy(h->own_stream);
+}
+
+// the continuous callback's per-member event lists for max_events events: times cc_t, counts cc_n and, for the family's own
+// conditions (words = true), the event words cc_ev
+int32_t cc_lists(Handle* h, int32_t max_events, bool words) {
+    const size_t N = (size_t)h->cfg.N, E = (size_t)max_events;
+    if (E != (size_t)h->cc_maxev || !h->d_cc_t) {
+        cudaFree(h->d_cc_t); cudaFree(h->d_cc_n); cudaFree(h->d_cc_ev); h->d_cc_t = nullptr; h->d_cc_n = nullptr; h->d_cc_ev = nullptr; h->cc_on = false;
+        CUDA_TRY(h, cudaMalloc(&h->d_cc_t, E * N * sizeof(double)));
+        CUDA_TRY(h, cudaMalloc(&h->d_cc_n, N * sizeof(int32_t)));
+    }
+    if (words && !h->d_cc_ev) CUDA_TRY(h, cudaMalloc(&h->d_cc_ev, E * N * sizeof(int32_t)));
+    CUDA_TRY(h, cudaMemsetAsync(h->d_cc_n, 0, N * sizeof(int32_t), h->stream));
+    return B200ADJ_OK;
+}
+void cc_release(Handle* h) {
+    cudaFree(h->d_cc_t); cudaFree(h->d_cc_n); cudaFree(h->d_cc_ev); h->d_cc_t = nullptr; h->d_cc_n = nullptr; h->d_cc_ev = nullptr;
+    h->cc_on = false; h->fe_nc = 0; h->have_forward = false;
 }
 
 // dp += coef_c .* p + coef_e per member (shared parameters: N times, once)
@@ -652,22 +672,15 @@ int32_t b200adj_set_continuous_callback(void* handle, int32_t enabled, int32_t i
     const b200adj_cfg& c = h->cfg;
     CUDA_TRY(h, cudaSetDevice(c.device));
     CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-    if (!enabled) {
-        cudaFree(h->d_cc_t); cudaFree(h->d_cc_n); h->d_cc_t = nullptr; h->d_cc_n = nullptr; h->cc_on = false; h->have_forward = false;
-        return B200ADJ_OK;
-    }
+    if (!enabled) { cc_release(h); return B200ADJ_OK; }
     if (h->path != Path::T5A || is_fixed_dt(h)) { h->err = "continuous callback: built for the adaptive Tsit5 stepper (F64)"; return B200ADJ_ERR_UNSUPPORTED; }
     if (int32_t rc = check_support(h, c.sensealg, h->nev > 0, true)) return rc;
     if (h->nev > 0) { h->err = "continuous callback together with preset-time events is not built"; return B200ADJ_ERR_UNSUPPORTED; }
     if (c.d > 4) { h->err = "continuous callback: d <= 4"; return B200ADJ_ERR_UNSUPPORTED; }
     if (idx < 0 || idx >= c.d || direction < -1 || direction > 1 || pcomp >= c.d || (pcomp >= 0 && (pparam < 0 || pparam >= c.P)) || max_events < 1 ||
         !std::isfinite(level) || !std::isfinite(psign)) { h->err = "continuous callback: bad idx / direction / pcomp / pparam / max_events"; return B200ADJ_ERR_INVALID; }
-    if ((size_t)max_events != (size_t)h->cc_maxev || !h->d_cc_t) {
-        cudaFree(h->d_cc_t); cudaFree(h->d_cc_n); h->d_cc_t = nullptr; h->d_cc_n = nullptr; h->cc_on = false;
-        CUDA_TRY(h, cudaMalloc(&h->d_cc_t, (size_t)max_events * (size_t)c.N * sizeof(double)));
-        CUDA_TRY(h, cudaMalloc(&h->d_cc_n, (size_t)c.N * sizeof(int32_t)));
-    }
-    CUDA_TRY(h, cudaMemsetAsync(h->d_cc_n, 0, (size_t)c.N * sizeof(int32_t), h->stream));
+    if (int32_t rc = cc_lists(h, max_events, false)) return rc;
+    h->fe_nc = 0;                     // the named condition and affect
     h->cc_on = true; h->cc_idx = idx; h->cc_dir = direction; h->cc_pcomp = pcomp < 0 ? -1 : pcomp; h->cc_pparam = pcomp < 0 ? 0 : pparam;
     h->cc_maxev = max_events; h->cc_level = level; h->cc_psign = psign;
     h->cc_lparam = -1; h->cc_lcoef = 0; h->cc_acomp = -1; h->cc_aparam = 0; h->cc_acoef = 0; h->cc_qcomp = -1; h->cc_qcoef = 1;   // set_continuous_callback_params adds them
@@ -682,6 +695,7 @@ int32_t b200adj_set_continuous_callback_params(void* handle, int32_t lparam, dou
     Handle* h = (Handle*)handle;
     const b200adj_cfg& c = h->cfg;
     if (!h->cc_on) { h->err = "continuous callback parameters: call b200adj_set_continuous_callback first"; return B200ADJ_ERR_STATE; }
+    if (h->fe_nc > 0) { h->err = "continuous callback parameters: the callback uses the family's own conditions and affect"; return B200ADJ_ERR_STATE; }
     if (lparam >= c.P || (acomp >= 0 && (acomp >= c.d || aparam < 0 || aparam >= c.P)) || !std::isfinite(lcoef) || !std::isfinite(acoef)) {
         h->err = "continuous callback parameters: bad lparam / acomp / aparam"; return B200ADJ_ERR_INVALID; }
     if (acomp >= 0 && acomp == h->cc_pcomp) { h->err = "continuous callback parameters: acomp is the component the parameter-scaled affect overwrites"; return B200ADJ_ERR_INVALID; }
@@ -704,6 +718,46 @@ int32_t b200adj_event_times(void* handle, int32_t* counts, double* times) {
     CUDA_TRY(h, cudaStreamSynchronize(h->stream));
     if (counts) CUDA_TRY(h, cudaMemcpy(counts, h->d_cc_n, (size_t)h->cfg.N * sizeof(int32_t), cudaMemcpyDeviceToHost));
     if (times) CUDA_TRY(h, cudaMemcpy(times, h->d_cc_t, (size_t)h->cc_maxev * (size_t)h->cfg.N * sizeof(double), cudaMemcpyDeviceToHost));
+    return B200ADJ_OK;
+}
+
+int32_t b200adj_family_conditions(int32_t family, int32_t* nc) {
+    if (!nc) return B200ADJ_ERR_INVALID;
+    if (const FamilyVTable* vt = family_lookup(family)) { *nc = vt->nc; return B200ADJ_OK; }
+    for (const FamDims& f : OWN_DISPATCH_FAMILIES)
+        if (f.id == family) { *nc = 0; return B200ADJ_OK; }
+    return B200ADJ_ERR_INVALID;
+}
+
+int32_t b200adj_set_family_events(void* handle, int32_t enabled, int32_t nc, const int32_t* direction, int32_t max_events) {
+    if (!handle) return B200ADJ_ERR_INVALID;
+    Handle* h = (Handle*)handle;
+    const b200adj_cfg& c = h->cfg;
+    CUDA_TRY(h, cudaSetDevice(c.device));
+    CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+    if (!enabled) { cc_release(h); return B200ADJ_OK; }
+    const FamilyVTable* vt = family_lookup(c.rhs_family);
+    if (!vt || vt->nc < 1) { h->err = "family events: the family carries no conditions (build its plug-in with B200ADJ_FAMILY_HAS_EVENTS)"; return B200ADJ_ERR_UNSUPPORTED; }
+    if (h->path != Path::T5A || is_fixed_dt(h)) { h->err = "family events: built for the adaptive Tsit5 stepper (F64)"; return B200ADJ_ERR_UNSUPPORTED; }
+    if (h->nev > 0) { h->err = "family events together with preset-time events are not built"; return B200ADJ_ERR_UNSUPPORTED; }
+    if (int32_t rc = check_support(h, c.sensealg, false, true)) return rc;
+    if (nc != vt->nc || !direction || max_events < 1) { h->err = "family events: nc differs from the family's, null direction or max_events < 1"; return B200ADJ_ERR_INVALID; }
+    for (int k = 0; k < nc; k++)
+        if (direction[k] < -1 || direction[k] > 1) { h->err = "family events: a direction is outside {-1, 0, 1}"; return B200ADJ_ERR_INVALID; }
+    if (int32_t rc = cc_lists(h, max_events, true)) return rc;
+    h->cc_on = true; h->cc_maxev = max_events; h->fe_nc = nc;
+    for (int k = 0; k < 8; k++) h->fe_dir[k] = k < nc ? direction[k] : 0;
+    h->have_forward = false;
+    return B200ADJ_OK;
+}
+
+int32_t b200adj_event_flags(void* handle, int32_t* ev) {
+    if (!handle || !ev) return B200ADJ_ERR_INVALID;
+    Handle* h = (Handle*)handle;
+    if (!h->cc_on || h->fe_nc < 1 || !h->have_forward) { h->err = "event_flags: needs family events and a forward pass"; return B200ADJ_ERR_STATE; }
+    CUDA_TRY(h, cudaSetDevice(h->cfg.device));
+    CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+    CUDA_TRY(h, cudaMemcpy(ev, h->d_cc_ev, (size_t)h->cc_maxev * (size_t)h->cfg.N * sizeof(int32_t), cudaMemcpyDeviceToHost));
     return B200ADJ_OK;
 }
 

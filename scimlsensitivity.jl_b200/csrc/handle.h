@@ -82,6 +82,9 @@ struct Handle {
     double cc_level = 0, cc_psign = 1, cc_scale[4] = {1, 1, 1, 1}, cc_shift[4] = {0, 0, 0, 0};
     int cc_lparam = -1, cc_acomp = -1, cc_aparam = 0, cc_qcomp = -1; double cc_lcoef = 0, cc_acoef = 0, cc_qcoef = 1;      // b200adj_set_continuous_callback_params
     double* d_cc_t = nullptr; int32_t* d_cc_n = nullptr;
+    // the callback's family mode (b200adj_set_family_events): fe_nc > 0 conditions of the family, their directions, and the
+    // event words cc_ev[cc_maxev][N] of the events found
+    int fe_nc = 0; int32_t fe_dir[8] = {0}; int32_t* d_cc_ev = nullptr;
     int rev_block = 0; const void* rev_block_kernel = nullptr;      // adaptive Tsit5 reverse kernel: block size chosen per instantiation (disp_t5a.inc)
     bool have_forward = false;
     bool noise_valid = false;
@@ -149,6 +152,7 @@ struct FamilyVTable {
     int (*ros_rev)(Handle*, const RosArgs&);
     int (*fwd_f32)(Handle*, const OdeFwdArgsT<float>&);     // fixed-step Tsit5 in F32 (built-in LV / Lorenz; null elsewhere)
     int (*rev_f32)(Handle*, const OdeRevArgsT<float>&);
+    int32_t nc;                   // conditions of the family's own state-dependent event (B200ADJ_FAMILY_HAS_EVENTS); 0: none
 };
 constexpr uint32_t B200ADJ_PLUGIN_ABI = 0x00020000u ^ (uint32_t)sizeof(Handle) ^ ((uint32_t)sizeof(OdeRevArgs) << 8) ^
                                         ((uint32_t)sizeof(T5aArgs) << 16) ^ ((uint32_t)sizeof(FamilyVTable) << 24);

@@ -53,7 +53,18 @@ struct T5aArgs {
     double C[7];
     double BT[7];           // embedded error weights b - bhat
     double R[7][4];         // dense-output polynomials: b_j(theta) = sum_m R[j][m] theta^(m+1)
+    // family events (VectorContinuousCallback, b200adj_set_family_events): the continuous callback's conditions and affect are
+    // the ones compiled into the family struct (Fam::NC, condition, condition_grad, affect, affect_vjp; family_plugin.inc).
+    // fe_nc > 0 selects them; fe_dir[c] is the direction of condition c (-1 down, +1 up, 0 both).  The forward kernel stores
+    // with each event time of cc_t its event word cc_ev[cc_maxev][N]: bit 2c = condition c fired, bit 2c + 1 = it crossed upwards.
+    int32_t fe_nc, fe_dir[8];
+    int32_t* cc_ev;
 };
+
+// a family struct carries conditions and an affect (family_plugin.inc specialises this for B200ADJ_FAMILY_HAS_EVENTS)
+template <class Fam> struct FamilyEvents { static constexpr bool value = false; };
+__host__ __device__ constexpr uint32_t fe_fired(uint32_t word, int c) { return (word >> (2 * c)) & 1u; }
+__host__ __device__ constexpr uint32_t fe_upward(uint32_t word, int c) { return (word >> (2 * c + 1)) & 1u; }
 
 __device__ __forceinline__ void t5_weights(const T5aArgs& a, double th, double* w) {
 #pragma unroll
@@ -223,7 +234,89 @@ __device__ __forceinline__ double t5_pick(const double* v, int idx) {
     return r;
 }
 
-template <class Fam, bool SHARED_P, bool CC = false>
+// Condition policy of the state-dependent event: NC conditions g_c(y, p, t), each with its direction -- here the conditions
+// compiled into the family (b200adj_set_family_events).  (The named condition u[cc_idx] - level keeps its own scalar loop in
+// t5a_forward_kernel: routed through t5_find_event it compiles to different SASS, and its kernels are pinned.)
+template <class Fam>
+struct T5FamilyCond {
+    static constexpr int NC = Fam::NC;
+    const T5aArgs& a;
+    __device__ __forceinline__ void operator()(const double* y, const double* p, double t, double* g) const { Fam::condition(y, p, t, g); }
+    __device__ __forceinline__ int dir(int c) const { return a.fe_dir[c]; }
+};
+
+// Event search on one accepted step [t, t + h] (k1..k7 in registers, un = the end point): the conditions are evaluated on the
+// dense output y(theta) at theta = j / 10 (interp_points = 10 of ContinuousCallback: a long step may hold a whole flight);
+// the first sample interval in which any condition changes sign in its direction holds the event.  Every condition that
+// crosses there is bisected to the last bit; theta* is the smallest root and the conditions whose root has the same bits
+// fire together.  Conditions in `skip` (those that fired at the event the step starts on, ~0 with a random sign) take their
+// side from the first sample instead.  Returns the event word (bit 2c fired, bit 2c + 1 upwards; 0 = no event) and theta*.
+template <int D, class Cond>
+__device__ __forceinline__ uint32_t t5_find_event(const T5aArgs& a, const Cond& cond, const double* u, const double* un,
+                                                  const double (*k)[D], const double* p, double t, double h, uint32_t skip, double* thstar) {
+    constexpr int NC = Cond::NC;
+    auto conds_at = [&](double th, double* g) {         // the full dense output y(theta), once per sample
+        double y[D], w[7];
+        t5_weights(a, th, w);
+#pragma unroll
+        for (int j = 0; j < D; j++) {
+            double acc = 0.0;
+#pragma unroll
+            for (int s = 0; s < 7; s++) acc += w[s] * k[s][j];
+            y[j] = u[j] + h * acc;
+        }
+        cond(y, p, t + th * h, g);
+    };
+    double gprev[NC], gj[NC], thprev = 0.0, lo = 0.0, hi = 1.0;
+    cond(u, p, t, gprev);
+    uint32_t cross = 0;
+    for (int j = 1; j <= 10 && !cross; j++) {
+        const double th = j == 10 ? 1.0 : 0.1 * j;
+        if (j == 10) cond(un, p, t + h, gj); else conds_at(th, gj);
+#pragma unroll
+        for (int c = 0; c < NC; c++) {
+            if (j == 1 && ((skip >> c) & 1u)) continue;
+            const int dr = cond.dir(c);
+            if ((dr <= 0 && gprev[c] > 0 && gj[c] <= 0) || (dr >= 0 && gprev[c] < 0 && gj[c] >= 0)) cross |= 1u << c;
+        }
+        if (cross) { lo = thprev; hi = th; }
+        else {
+#pragma unroll
+            for (int c = 0; c < NC; c++) gprev[c] = gj[c];
+            thprev = th;
+        }
+    }
+    if (!cross) return 0u;
+    double root[NC], ts = 2.0;
+    bool any = false;
+#pragma unroll
+    for (int c = 0; c < NC; c++) {
+        root[c] = 2.0;
+        if (NC > 1 && !((cross >> c) & 1u)) continue;
+        // bisection to the last bit; the root is the first theta on the far side
+        const bool pos = gprev[c] > 0;
+        double l = lo, r = hi;
+        for (int it = 0; it < 200; it++) {
+            const double mid = 0.5 * (l + r);
+            if (!(mid > l && mid < r)) break;
+            double gm[NC];
+            conds_at(mid, gm);
+            if ((gm[c] > 0) == pos && gm[c] != 0) l = mid; else r = mid;
+        }
+        root[c] = r;
+        ts = any ? fmin(ts, r) : r;
+        any = true;
+    }
+    uint32_t word = 0;
+#pragma unroll
+    for (int c = 0; c < NC; c++)
+        if (root[c] == ts) word |= (1u << (2 * c)) | ((gprev[c] < 0 ? 1u : 0u) << (2 * c + 1));
+    *thstar = ts;
+    return word;
+}
+
+// CC: state-dependent event; FE (with CC): its conditions and affect are those of the family (T5FamilyCond), else named
+template <class Fam, bool SHARED_P, bool CC = false, bool FE = false>
 __global__ void __launch_bounds__(256) t5a_forward_kernel(const __grid_constant__ T5aArgs a) {
     constexpr int D = Fam::D, P = Fam::P;
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -255,7 +348,8 @@ __global__ void __launch_bounds__(256) t5a_forward_kernel(const __grid_constant_
     const bool fixed = (a.flags & KF_FIXED_DT) != 0;      // constant step dt0, no error control (fixed-step Tsit5 with off-grid save times)
     bool after_event = false;                     // CC: the step starts on an event (condition ~0 with a random sign)
     int nfound = 0;
-    const double cc_lev = CC ? t5_cc_level<P>(a, p) : 0.0;
+    const double cc_lev = (CC && !FE) ? t5_cc_level<P>(a, p) : 0.0;
+    uint32_t fe_skip = 0, fe_word = 0;            // FE: conditions that fired at the event the step starts on; the event word
     // component cc_idx of the step's dense output at theta (k1..k7 in registers)
     auto cond_at = [&](double th, double hh) {
         double w[7];
@@ -288,7 +382,24 @@ __global__ void __launch_bounds__(256) t5a_forward_kernel(const __grid_constant_
         if (EEst <= 1.0) {
             double tn = last ? tend : t + h;
             bool at_event = !CC && last && ev < a.nev;
-            if (CC) {
+            if constexpr (FE) {
+                // the family's conditions (t5_find_event): right after an event the conditions that fired there take their
+                // side from the first sample; the step is redone up to theta* as below
+                double thstar = 1.0;
+                const uint32_t word = t5_find_event<D>(a, T5FamilyCond<Fam>{a}, u, un, k, p, t, h, fe_skip, &thstar);
+                fe_skip = 0;
+                if (word) {
+                    const double hh = thstar * h;
+                    t5_step<D>(a, rhs, t, hh, u, k, un);
+                    tn = t + hh;
+                    at_event = true;
+                    if (nfound >= a.cc_maxev) { stat = 3; break; }
+                    a.cc_t[(int64_t)nfound * N + i] = tn;
+                    a.cc_ev[(int64_t)nfound * N + i] = (int32_t)word;
+                    fe_word = word;
+                    nfound++;
+                }
+            } else if (CC) {
                 // sign changes of the condition on the dense output, sampled at theta = j / 10 (interp_points = 10 of
                 // ContinuousCallback: a long step may hold a whole flight); right after an event the first sample decides the side
                 double gprev = t5_pick<D>(u, a.cc_idx) - cc_lev, thprev = 0.0, lo = 0.0, hi = 1.0;
@@ -362,7 +473,19 @@ __global__ void __launch_bounds__(256) t5a_forward_kernel(const __grid_constant_
             }
             if (at_event) {
                 // affect!: the next step starts from the post-event state; k7 = f(u^-) stays with the step just stored
-                if (CC) {
+                if constexpr (FE) {
+                    // affect!(integrator, ev) of the family: ev[c] = +1 / -1 for a condition that crossed upwards / downwards
+                    int evs[Fam::NC];
+                    double up[D];
+#pragma unroll
+                    for (int c = 0; c < Fam::NC; c++) evs[c] = fe_fired(fe_word, c) ? (fe_upward(fe_word, c) ? 1 : -1) : 0;
+                    Fam::affect(evs, un, p, up);
+#pragma unroll
+                    for (int j = 0; j < D; j++) un[j] = up[j];
+                    fe_skip = 0;
+#pragma unroll
+                    for (int c = 0; c < Fam::NC; c++) fe_skip |= fe_fired(fe_word, c) << c;
+                } else if (CC) {
                     double sc[D], sh[D];
                     t5_cc_affect<D, P>(a, p, sc, sh);
 #pragma unroll
@@ -431,7 +554,7 @@ __global__ void __launch_bounds__(256) t5a_forward_kernel(const __grid_constant_
 // (A register cap -- __maxnreg__(144): 14 warps per SM, the 65 536-member C1 shard in ONE wave instead of two -- was measured
 // twice and rejected: 8.9 ms against 7.25 ms uncapped.  Block sizes 32 / 64 / 128 (8 to 11 resident warps per SM) all give
 // 7.25 ms: the time is two rounds of a latency-bound per-warp chain, see DESIGN.md 4.4.)
-template <class Fam, int SA, bool SHARED_P, int COST, bool CC = false>
+template <class Fam, int SA, bool SHARED_P, int COST, bool CC = false, bool FE = false>
 __global__ void __launch_bounds__(256) t5a_reverse_kernel(const __grid_constant__ T5aArgs a) {
     constexpr int D = Fam::D, P = Fam::P, L = (SA == SA_INTERP) ? D + P : (SA == SA_BACKSOLVE ? 2 * D + P : D);
     constexpr int YO = (SA == SA_BACKSOLVE) ? D + P : 0;          // offset of y inside z (Backsolve)
@@ -517,7 +640,42 @@ __global__ void __launch_bounds__(256) t5a_reverse_kernel(const __grid_constant_
     // solution (the reference keeps it as `uleft` of the TrackedAffect).  Runs after the checkpoint reset and the loss jump.
     auto event_if_at = [&](double tt) {
         while (evc >= 0 && fabs(evt(evc) - tt) <= EPS100 * fmax(fabs(tt), 1.0)) {
-            if constexpr (CC) {
+            if constexpr (FE) {
+                // state-dependent event of the family's conditions and affect (the implicit event-time correction of
+                // src/callback_tracking.jl:232-480): with u+ = a(u-, p), c = the lowest condition that fired, g_c(u-, p, tau) = 0,
+                //   (mu_u, mu_p) = ((da/du)'lam+, (da/dp)'lam+),  den = dg/du . f(u-) + dg/dt,  w = mu_u . f(u-) - lam+ . f(u+)
+                //   lam- = mu_u - dg/du (w / den),  dG/dp += mu_p - dg/dp (w / den)
+                // For g = u_i - level - lcoef p_k and a diagonal affect this is the named formula of the branch below.
+                constexpr int NC = Fam::NC;
+                double um[D], up[D], fm[D], fp[D], mu[D], mp[P], gu[D], gp[P];
+                const double tau = evt(evc);
+                sol.eval(tau, false, um); sol.eval(tau, true, up);
+                Fam::f(um, p, fm); Fam::f(up, p, fp);
+                const uint32_t word = (uint32_t)a.cc_ev[(int64_t)evc * N + i];
+                int evs[NC], cf = 0;
+#pragma unroll
+                for (int c = NC - 1; c >= 0; c--) {
+                    evs[c] = fe_fired(word, c) ? (fe_upward(word, c) ? 1 : -1) : 0;
+                    if (evs[c]) cf = c;
+                }
+                Fam::affect_vjp(evs, um, p, z, mu, mp);
+                const double gt = Fam::condition_grad(cf, um, p, tau, gu, gp);
+                double den = gt, w = 0.0;
+#pragma unroll
+                for (int j = 0; j < D; j++) { den += gu[j] * fm[j]; w += mu[j] * fm[j] - z[j] * fp[j]; }
+                const double r = w / den;
+#pragma unroll
+                for (int q = 0; q < P; q++) {
+                    const double dq = mp[q] - gp[q] * r;
+                    if (SA == SA_INTERP || SA == SA_BACKSOLVE) z[D + (L > D ? q : 0)] += dq; else acc[q] += dq;
+                }
+#pragma unroll
+                for (int j = 0; j < D; j++) z[j] = mu[j] - gu[j] * r;
+                if (SA == SA_BACKSOLVE) {
+#pragma unroll
+                    for (int j = 0; j < D; j++) z[YO + j] = um[j];
+                }
+            } else if constexpr (CC) {
                 // state-dependent event time (the implicit correction of src/callback_tracking.jl:232-480): with u+ = A u- + c,
                 // g(u-) = 0:  lam- = A'lam+ - e_ci [(A f- - f+)'lam+] / f-[ci],   dG/dp += (dA/dp u-)'lam+
                 double um[D], up[D], fm[D], fp[D], sc[D], sh[D];

@@ -6,7 +6,7 @@ is in libb200adj.so.
 import numpy as np
 
 from . import _lib
-from .problems import FAMILIES, AffineCost, ParamAffine
+from .problems import FAMILIES, FAMILY_CONDITIONS, AffineCost, ParamAffine, VectorContinuousCallback
 
 
 def _is_torch(x):
@@ -156,10 +156,18 @@ class DeviceEnsemble:
         self.handle.set_event_param_shift(comp, param, coef)
 
     def set_continuous_callback(self, cb):
-        """State-dependent event (problems.ContinuousCallback) of the hybrid system; call before forward().  None removes it."""
+        """State-dependent event (problems.ContinuousCallback, or problems.VectorContinuousCallback with the conditions and
+        affect of the family) of the hybrid system; call before forward().  None removes it."""
         if cb is None:
             self.handle.set_continuous_callback(0, enabled=False)
             self.continuous_callback = None
+            return
+        if isinstance(cb, VectorContinuousCallback):
+            if tuple(cb.save_positions) != (False, False):
+                raise NotImplementedError("VectorContinuousCallback: save_positions = (false, false) is the mode carried on the device")
+            nc = FAMILY_CONDITIONS.get(self.family, 0)
+            self.handle.set_family_events(nc, cb.directions(nc) if nc else np.zeros(0, np.int32), cb.max_events)   # nc = 0: refused
+            self.continuous_callback = cb
             return
         if tuple(cb.save_positions) != (False, False):
             raise NotImplementedError("ContinuousCallback: save_positions = (false, false) is the mode carried on the device")
@@ -177,6 +185,17 @@ class DeviceEnsemble:
     def event_times(self):
         """-> (counts[N], times[max_events, N]): the event lists found by the last forward pass."""
         return self.handle.event_times(self.N, self.continuous_callback.max_events)
+
+    def event_flags(self):
+        """VectorContinuousCallback: -> ev[max_events, NC, N] (int8) of the last forward pass, the `ev` each affect saw:
+        +1 / -1 for a condition that fired crossing upwards / downwards, 0 for one that did not; 0 past a member's events."""
+        nc = FAMILY_CONDITIONS.get(self.family, 0)
+        counts, _ = self.handle.event_times(self.N, self.continuous_callback.max_events)
+        words = self.handle.event_flags(self.N, self.continuous_callback.max_events)
+        words[np.arange(words.shape[0])[:, None] >= counts[None, :]] = 0
+        fired = (words[:, None, :] >> (2 * np.arange(nc))[None, :, None]) & 1
+        up = (words[:, None, :] >> (2 * np.arange(nc) + 1)[None, :, None]) & 1
+        return (fired * (2 * up - 1)).astype(np.int8)
 
     def set_reverse(self, sensealg, cost=None, no_start=False, checkpointing=True, ckpt_every_step=False, t=None, dgdp=None):
         """Re-target the next reverse pass (sensealg / cost / save times) without re-running the forward pass.

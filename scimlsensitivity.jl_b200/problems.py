@@ -18,6 +18,8 @@ FAMILIES = {
     "relax": (1, 2, 0),          # u' = p[0] - u; p = [steady state, injected amount] (test/Callbacks2/continuous_callbacks.jl:317-324)
     "mlp": (2, 4482, 0),         # 2 -> 64 -> 64 -> 2 tanh MLP, p = [W1, b1, W2, b2, W3, b3] column-major flattened
 }
+# conditions compiled into a registered plug-in family (VectorContinuousCallback); families not listed have none
+FAMILY_CONDITIONS = {}
 
 
 class AdjointSensitivityParameterCompatibilityError(TypeError):
@@ -197,6 +199,33 @@ class ContinuousCallback:
         sh = None if self.shift is None else np.asarray(self.shift, dtype=np.float64).tobytes()
         return ("cc", self.idx, self.level, self.direction, sc, sh, self.p_comp, self.p_param, self.p_sign, self.max_events,
                 self.level_param, self.level_coef, self.add_comp, self.add_param, self.add_coef, self.sq_comp, self.sq_coef)
+
+
+@dataclass(frozen=True)
+class VectorContinuousCallback:
+    """VectorContinuousCallback(condition, affect!, NC) whose condition(out, u, t, integrator) and affect!(integrator, ev) are
+    the ones compiled into the problem's family (a plug-in built with has_events=True: csrc/family_plugin.inc,
+    examples/vector_callback_families.cuh); with NC = 1 it is a ContinuousCallback with a general condition.  The reference's
+    treatment: src/callback_tracking.jl:232-480.
+      direction: -1 (a condition fires when it crosses zero downwards only), +1 (upwards only) or 0 (both); a scalar or one
+                 entry per condition
+      max_events: per-member capacity of the event list (status 3 when exceeded)
+    save_positions = (false, false) only; every ensemble member finds its own events on the device, and the conditions whose
+    crossings land on the same bits fire together (ev has one non-zero entry per condition that fired)."""
+    direction: Any = 0
+    max_events: int = 64
+    save_positions: Tuple[bool, bool] = (False, False)
+
+    def directions(self, nc):
+        d = np.asarray(self.direction, dtype=np.int32).reshape(-1)
+        if d.size == 1:
+            d = np.full(nc, d[0], dtype=np.int32)
+        if d.shape != (nc,):
+            raise ValueError(f"VectorContinuousCallback: direction must be a scalar or have {nc} entries")
+        return np.ascontiguousarray(d)
+
+    def key(self):
+        return ("vcc", np.asarray(self.direction, dtype=np.int32).tobytes(), self.max_events)
 
 
 def saveat_to_times(saveat, tspan):
