@@ -229,6 +229,7 @@ template <class A> A dense_args(Handle* h) {
 T5aArgs t5a_args(Handle* h) {
     T5aArgs a = dense_args<T5aArgs>(h);
     a.dt0 = h->cfg.dt;
+    a.status = h->r_status;
     memcpy(a.A, TSIT5_A, sizeof(TSIT5_A)); memcpy(a.C, TSIT5_C, sizeof(TSIT5_C)); memcpy(a.BT, TSIT5_BT, sizeof(TSIT5_BT));
     tsit5_weights(0.0, nullptr, a.R);
     if (h->cont_on) for (int j = 0; j < 4; j++) { a.cont_a[j] = h->cont_av[j]; a.cont_b[j] = h->cont_bv[j]; }
@@ -255,7 +256,7 @@ void free_all(Handle* h) {
     cudaFree(h->d_kst); cudaFree(h->d_adj_dense); cudaFree(h->d_trace); cudaFree(h->d_ckpt); cudaFree(h->d_noise); cudaFree(h->d_partials); cudaFree(h->d_ticket); cudaFree(h->d_save_of_step); cudaFree(h->d_fwd_save_of_step); cudaFree(h->d_fwd_saveat);
     cudaFree(h->s_u0); cudaFree(h->s_p); cudaFree(h->s_saved); cudaFree(h->s_dLdu); cudaFree(h->s_du0); cudaFree(h->s_dp); cudaFree(h->s_dW);
     cudaFree(h->d_cc_t); cudaFree(h->d_cc_n); cudaFree(h->d_cc_ev);
-    cudaFree(h->s_status); cudaFree(h->d_event_of_step); cudaFree(h->d_ev_ac); cudaFree(h->d_ev_ak); cudaFree(h->d_ev_af); cudaFree(h->d_ev_t); cudaFree(h->d_ev_s); cudaFree(h->d_ev_c); cudaFree(h->d_ev_ps); cudaFree(h->d_ev_pc);
+    cudaFree(h->s_status); cudaFree(h->r_status); cudaFree(h->d_event_of_step); cudaFree(h->d_ev_ac); cudaFree(h->d_ev_ak); cudaFree(h->d_ev_af); cudaFree(h->d_ev_t); cudaFree(h->d_ev_s); cudaFree(h->d_ev_c); cudaFree(h->d_ev_ps); cudaFree(h->d_ev_pc);
     if (h->own_stream) cudaStreamDestroy(h->own_stream);
 }
 
@@ -445,6 +446,7 @@ int32_t b200adj_create(const b200adj_cfg* cfg, void** handle) {
         if (t5a) {      // member-major records (u_n, k1..k7, t_n, h, 1/h, t_{n+1}) and knots: tsit5_adaptive.cuh
             CREATE_TRY(cudaMalloc(&h->r_ftT, N * (MS + 1) * e));
             CREATE_TRY(cudaMalloc(&h->r_frecT, N * (MS + 1) * (size_t)(8 * d + 4) * e));
+            CREATE_TRY(cudaMalloc(&h->r_status, N * sizeof(int32_t)));
         } else {        // Rosenbrock23: step-major knots, states and the 2 dense-output stages
             CREATE_TRY(cudaMalloc(&h->r_ft, (MS + 1) * N * e));
             CREATE_TRY(cudaMalloc(&h->r_fu, (MS + 1) * d * N * e));
@@ -822,12 +824,17 @@ int32_t b200adj_forward(void* handle, const void* u0, const void* p, const void*
     const FamilyVTable* vt = family_lookup(c.rhs_family);      // the ODE paths' launchers
     int rc = 0;
     if (is_adaptive(h)) {
-        auto fwd = [&](auto a, auto fn) {
+        auto fwd = [&](auto a, auto fn, int32_t* st) {
             a.saveat = h->d_fwd_saveat; a.K = h->fwd_K;
-            a.u0 = du0; a.p = dp; a.saved = h->fwd_K > 0 ? dsaved : nullptr; a.status = dstatus;
+            a.u0 = du0; a.p = dp; a.saved = h->fwd_K > 0 ? dsaved : nullptr; a.status = st;
             return launch(fn, h, a);
         };
-        rc = h->path == Path::T5A ? fwd(t5a_args(h), vt->t5a_fwd) : fwd(dense_args<RosArgs>(h), vt->ros_fwd);
+        if (h->path == Path::T5A) {
+            // the status always lands in the handle (the reverse pass returns NaN for a member that stopped early), then in
+            // the caller's array
+            rc = fwd(t5a_args(h), vt->t5a_fwd, h->r_status);
+            if (!rc && dstatus) CUDA_TRY(h, cudaMemcpyAsync(dstatus, h->r_status, N * sizeof(int32_t), cudaMemcpyDeviceToDevice, h->stream));
+        } else rc = fwd(dense_args<RosArgs>(h), vt->ros_fwd, dstatus);
     } else if (h->path == Path::MLP) {
         rc = mlp_forward_dispatch(h, du0, dp, h->fwd_K > 0 ? dsaved : nullptr, dstatus);
     } else if (h->path == Path::FIXED && c.dtype == B200ADJ_F32) {

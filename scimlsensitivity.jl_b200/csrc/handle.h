@@ -73,6 +73,7 @@ struct Handle {
     // staging (buffers_on_device == 0)
     double *s_u0 = nullptr, *s_p = nullptr, *s_saved = nullptr, *s_dLdu = nullptr, *s_du0 = nullptr, *s_dp = nullptr, *s_dW = nullptr;
     int32_t* s_status = nullptr;
+    int32_t* r_status = nullptr;      // T5A: per-member status of the last forward pass, whether or not the caller asked for it (the reverse pass reads it)
     const double* cur_p = nullptr;    // device pointer to p valid between forward and reverse
     int32_t* d_ev_ac = nullptr; int32_t* d_ev_ak = nullptr; double* d_ev_af = nullptr;      // b200adj_set_event_param_shift
     int32_t* d_event_of_step = nullptr;     // fixed-step Tsit5: event index at grid point n, or -1

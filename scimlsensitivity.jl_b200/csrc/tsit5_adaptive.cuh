@@ -250,10 +250,13 @@ struct T5FamilyCond {
 // the first sample interval in which any condition changes sign in its direction holds the event.  Every condition that
 // crosses there is bisected to the last bit; theta* is the smallest root and the conditions whose root has the same bits
 // fire together.  Conditions in `skip` (those that fired at the event the step starts on, ~0 with a random sign) take their
-// side from the first sample instead.  Returns the event word (bit 2c fired, bit 2c + 1 upwards; 0 = no event) and theta*.
+// side from the first sample instead.  Returns the event word (bit 2c fired, bit 2c + 1 upwards; 0 = no event) and theta*;
+// *pending gets the same bits for the conditions that cross in that interval but whose roots have other bits
+// (t5_fire_reached decides them once the step is redone).
 template <int D, class Cond>
 __device__ __forceinline__ uint32_t t5_find_event(const T5aArgs& a, const Cond& cond, const double* u, const double* un,
-                                                  const double (*k)[D], const double* p, double t, double h, uint32_t skip, double* thstar) {
+                                                  const double (*k)[D], const double* p, double t, double h, uint32_t skip, double* thstar,
+                                                  uint32_t* pending) {
     constexpr int NC = Cond::NC;
     auto conds_at = [&](double th, double* g) {         // the full dense output y(theta), once per sample
         double y[D], w[7];
@@ -307,11 +310,30 @@ __device__ __forceinline__ uint32_t t5_find_event(const T5aArgs& a, const Cond& 
         ts = any ? fmin(ts, r) : r;
         any = true;
     }
+    uint32_t word = 0, pend = 0;
+#pragma unroll
+    for (int c = 0; c < NC; c++) {
+        const uint32_t bits = (1u << (2 * c)) | ((gprev[c] < 0 ? 1u : 0u) << (2 * c + 1));
+        if (root[c] == ts) word |= bits;
+        else if ((cross >> c) & 1u) pend |= bits;
+    }
+    *thstar = ts;
+    *pending = pend;
+    return word;
+}
+
+// The conditions of `pending` whose value at the end point un of the redone step (time tn) has reached their far side or
+// zero fire with the event.  The next step starts from un, and a condition that starts there on its far side or on zero can
+// never satisfy the crossing test: a root a few ulps after theta* would otherwise be lost (its affect silently skipped).
+template <class Fam>
+__device__ __forceinline__ uint32_t t5_fire_reached(const double* un, const double* p, double tn, uint32_t pending) {
+    if (!pending) return 0u;
+    double g[Fam::NC];
+    Fam::condition(un, p, tn, g);
     uint32_t word = 0;
 #pragma unroll
-    for (int c = 0; c < NC; c++)
-        if (root[c] == ts) word |= (1u << (2 * c)) | ((gprev[c] < 0 ? 1u : 0u) << (2 * c + 1));
-    *thstar = ts;
+    for (int c = 0; c < Fam::NC; c++)
+        if (fe_fired(pending, c) && (fe_upward(pending, c) ? g[c] >= 0 : g[c] <= 0)) word |= pending & (3u << (2 * c));
     return word;
 }
 
@@ -386,12 +408,17 @@ __global__ void __launch_bounds__(256) t5a_forward_kernel(const __grid_constant_
                 // the family's conditions (t5_find_event): right after an event the conditions that fired there take their
                 // side from the first sample; the step is redone up to theta* as below
                 double thstar = 1.0;
-                const uint32_t word = t5_find_event<D>(a, T5FamilyCond<Fam>{a}, u, un, k, p, t, h, fe_skip, &thstar);
+                uint32_t pend = 0;
+                uint32_t word = t5_find_event<D>(a, T5FamilyCond<Fam>{a}, u, un, k, p, t, h, fe_skip, &thstar, &pend);
                 fe_skip = 0;
                 if (word) {
-                    const double hh = thstar * h;
+                    // an event never lands on the time of the one before (a root a few ulps into the step, right after an
+                    // event): the reverse pass tells events and their dense intervals apart by their times
+                    double hh = thstar * h;
+                    if (!(t + hh > t)) hh = fmax(fabs(t), 1e-300) * 2.220446049250313e-16;      // >= one ulp of t
                     t5_step<D>(a, rhs, t, hh, u, k, un);
                     tn = t + hh;
+                    word |= t5_fire_reached<Fam>(un, p, tn, pend);
                     at_event = true;
                     if (nfound >= a.cc_maxev) { stat = 3; break; }
                     a.cc_t[(int64_t)nfound * N + i] = tn;
@@ -611,7 +638,9 @@ __global__ void __launch_bounds__(256) t5a_reverse_kernel(const __grid_constant_
     // CC: this member's own event list, found by the forward solve
     auto evt = [&](int e) { return CC ? a.cc_t[(int64_t)e * N + i] : a.ev_t[e]; };
     int cur = a.K - 1, nrev = 0, ck = sol.n, evc = (CC ? a.cc_n[i] : a.nev) - 1;
-    bool fsal_ok = false, overflow = false;
+    // a member whose forward solve stopped before t1 (status 1 / 2 / 3) has records only up to the break: NaN, as for a
+    // reverse solve that overflows, not the gradient of a trajectory that was never solved
+    bool fsal_ok = false, overflow = a.status[i] != 0;
     const bool ckpt_on = !(a.flags & KF_NO_CHECKPOINTING), every = (a.flags & KF_CKPT_EVERY_STEP);
     if (SA == SA_BACKSOLVE) {
 #pragma unroll
@@ -778,7 +807,7 @@ __global__ void __launch_bounds__(256) t5a_reverse_kernel(const __grid_constant_
     double h = a.dt0 > 0 ? -a.dt0 : -1e-4 * (T - t0), qold = 1e-4;
     const bool fixed = (a.flags & KF_FIXED_DT) != 0;
     long iters = 0;
-    while (t > t0 && sol.n > 0) {
+    while (!overflow && t > t0 && sol.n > 0) {
         if (++iters > 50000000L || (SA == SA_QUAD && nrev >= a.maxs)) { overflow = true; break; }
         double tstop = t0;
         if (cur >= 0 && a.saveat[cur] < t && a.saveat[cur] > tstop) tstop = a.saveat[cur];
