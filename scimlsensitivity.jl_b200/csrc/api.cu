@@ -428,7 +428,7 @@ int32_t b200adj_create(const b200adj_cfg* cfg, void** handle) {
     h->grid = (int)((cfg->N + block - 1) / block);
     h->nsm = nsm; h->qgrid = quad_grid(cfg->N, nsm);
     h->qpartials_blocks = (size_t)h->qgrid + 1;                              // quadrature kernels: persistent grid
-    h->maxseg = ros ? 2 * maxs : 4096;                                       // quadgk segment capacity per data interval (multiple of 32)
+    h->maxseg = ros ? 2 * maxs : 4096;                                       // quadgk segment capacity per data interval (any value: quad_l1_blocks rounds up)
 #define CREATE_TRY(expr)                                                                         \
     do { cudaError_t _e = (expr); if (_e != cudaSuccess) {                                       \
         g_create_error = std::string(#expr) + ": " + cudaGetErrorString(_e);                     \

@@ -190,7 +190,7 @@ template <class K> inline int quad_launch_grid(const Handle* h, K kernel, size_t
     return h->qgrid < cap ? h->qgrid : cap;
 }
 int ensure_quad_buffers(Handle* h);      // api.cu: lazily allocates QuadratureAdjoint's dense solutions and the quadgk scratch
-inline size_t quad_smem(int maxseg) { return (size_t)QUAD_WARPS * (QUAD_SKEYS + (maxseg >> 5)) * sizeof(double); }
+inline size_t quad_smem(int maxseg) { return (size_t)QUAD_WARPS * (QUAD_SKEYS + quad_l1_blocks(maxseg)) * sizeof(double); }
 inline size_t quad_seg_doubles(int P, int maxseg, int qgrid) { return (size_t)qgrid * QUAD_WARPS * maxseg * (size_t)(((P + 4 + 3) / 4) * 4); }
 
 }  // namespace b200adj

@@ -167,16 +167,40 @@ __device__ __forceinline__ void gk15_pair(const F& f, const QuadBracket& br, dou
 
 // per-warp segment store.  Global (owned by this resident warp): seg[maxseg][SEGW] = (a, b, I[P], (flo, fhi), (rlo, rhi)) and
 // the keys (segment errors) of the segments >= QUAD_SKEYS.  Shared memory: skey[QUAD_SKEYS] = keys of the first segments (a data
-// interval rarely needs more), l1[maxseg / 32] = maxima of the 32-key blocks.
+// interval rarely needs more), l1[quad_l1_blocks(maxseg)] = maxima of the 32-key blocks.
 constexpr int QUAD_SKEYS = 512;
 struct QuadScratch { double* seg; double* key; double* skey; double* l1; int maxseg; };
+// block maxima one warp keeps: key maxseg - 1 lies in block (maxseg - 1) >> 5, so a partial last block needs its own entry
+__host__ __device__ constexpr int quad_l1_blocks(int maxseg) { return (maxseg + 31) >> 5; }
 
 __device__ __forceinline__ double pack2(int a, int b) { return __longlong_as_double(((long long)(unsigned int)a) | ((long long)b << 32)); }
 __device__ __forceinline__ void unpack2(double v, int* a, int* b) { const long long x = __double_as_longlong(v); *a = (int)(unsigned int)(x & 0xffffffffLL); *b = (int)(x >> 32); }
 
+// arg-max of the keys of segments 0 .. nseg-1: block maxima (shared memory), then the winning block's 32 keys.  Ties resolve to
+// the lowest segment index, as the oracle's linear scan: lane l scans blocks l, l+32, ... keeping its first maximum, and among
+// the lanes that hold the maximum the lowest BLOCK index wins (the lowest lane would prefer block 32 over block 1).
+// -> bi = winning block, w = winning segment, ew = its key; kv = this lane's key of block bi (0 past nseg).
+struct QuadPick { int bi, w; double ew, kv; };
+__device__ __forceinline__ QuadPick quad_queue_argmax(const QuadScratch& q, int nseg, int lane) {
+    const int nb = (nseg + 31) >> 5;
+    int bi = 0;
+    if (nb > 1) {
+        double bv = 0.0; int bl = -1;
+        for (int bb = lane; bb < nb; bb += 32) { const double v = q.l1[bb]; if (bl < 0 || v > bv) { bv = v; bl = bb; } }
+        const int src = warp_argmax_lane(bv, bl >= 0);
+        const long long mx = __double_as_longlong(__shfl_sync(0xffffffffu, bv, src));
+        bi = __reduce_min_sync(0xffffffffu, (unsigned)((bl >= 0 && __double_as_longlong(bv) == mx) ? bl : 0x7fffffff));
+    }
+    const int kidx = bi * 32 + lane;
+    const double kv = kidx < nseg ? (kidx < QUAD_SKEYS ? q.skey[kidx] : __ldcg(q.key + kidx)) : 0.0;
+    const int wl = warp_argmax_lane(kv, kidx < nseg);
+    return QuadPick{bi, bi * 32 + wl, __shfl_sync(0xffffffffu, kv, wl), kv};
+}
+
 // adaptive quadgk over [a,b] by one warp.  `root` = index bracket of the whole panel.  false = out of segment capacity.
 template <int P, class F>
 __device__ bool quadgk_warp(const F& f, const QuadBracket& root, double a, double b, double atol, double rtol, double* out, const QuadScratch& q, int lane) {
+    static_assert(P <= 12, "a segment record (a, b, I[P], two brackets) is stored by at most 16 lanes of a half warp");
     constexpr int SEGW = quad_segw<P>();
     const int half = lane >> 4, c = lane & 15;             // c: element of the segment record this lane stores
     double Ih[P], Itot[P], eh, Etot;
@@ -202,20 +226,10 @@ __device__ bool quadgk_warp(const F& f, const QuadBracket& root, double a, doubl
         nI = sqrt(nI);
         if (Etot <= fmax(atol, rtol * nI)) break;
         if (nseg + 1 > q.maxseg) { ok = false; break; }
-        // ---- arg-max of the segment errors: block maxima (shared memory), then the winning block's 32 keys ----
-        const int nb = (nseg + 31) >> 5;
-        int bi = 0;
-        if (nb > 1) {
-            double bv = 0.0; int bl = -1;
-            for (int bb = lane; bb < nb; bb += 32) { const double v = q.l1[bb]; if (bl < 0 || v > bv) { bv = v; bl = bb; } }
-            const int src = warp_argmax_lane(bv, bl >= 0);
-            bi = __shfl_sync(0xffffffffu, bl, src);
-        }
-        const int kidx = bi * 32 + lane;
-        const double kv = kidx < nseg ? (kidx < QUAD_SKEYS ? q.skey[kidx] : __ldcg(q.key + kidx)) : 0.0;
-        const int wl = warp_argmax_lane(kv, kidx < nseg);
-        const int w = bi * 32 + wl;
-        const double ew = __shfl_sync(0xffffffffu, kv, wl);
+        // ---- arg-max of the segment errors ----
+        const QuadPick pk = quad_queue_argmax(q, nseg, lane);
+        const int bi = pk.bi, w = pk.w;
+        const double ew = pk.ew, kv = pk.kv;
         // ---- the segment record (every lane reads the same addresses: broadcast loads) ----
         const double* sr = q.seg + (size_t)w * SEGW;
         const double aw = __ldcg(sr), bw = __ldcg(sr + 1);
@@ -325,9 +339,9 @@ __device__ __forceinline__ void quad_member_loop(int64_t N, int K, const double*
                                                  double* qseg, double* qkey, int maxseg, double* l1_smem, const MAKE& make, const SINK& sink) {
     const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
     const int64_t gw = (int64_t)blockIdx.x * QUAD_WARPS + wib, G = (int64_t)gridDim.x * QUAD_WARPS;
-    // dynamic shared memory of the block: [QUAD_WARPS][QUAD_SKEYS] keys, then [QUAD_WARPS][maxseg / 32] block maxima
+    // dynamic shared memory of the block: [QUAD_WARPS][QUAD_SKEYS] keys, then [QUAD_WARPS][quad_l1_blocks(maxseg)] block maxima
     const QuadScratch qs{qseg + (size_t)gw * maxseg * quad_segw<P>(), qkey + (size_t)gw * maxseg, l1_smem + (size_t)wib * QUAD_SKEYS,
-                         l1_smem + (size_t)QUAD_WARPS * QUAD_SKEYS + (size_t)wib * (maxseg >> 5), maxseg};
+                         l1_smem + (size_t)QUAD_WARPS * QUAD_SKEYS + (size_t)wib * quad_l1_blocks(maxseg), maxseg};
     for (int64_t i = gw; i < N; i += G) {
         double res[P], part[P];
 #pragma unroll
