@@ -338,6 +338,47 @@ __device__ __forceinline__ void reduce_dp(const double* acc, double* partials, R
     }
 }
 
+// dG/dp write-out of a reverse kernel: a shared p sums acc over the grid (reduce_dp; an inactive thread adds zeros, and every
+// thread of the block must arrive), a per-member p stores member i's row.
+template <int P, bool SHARED_P>
+__device__ __forceinline__ void store_dp(double* acc, bool active, int64_t i, int64_t N, double* dp_members, double* partials, double* dp,
+                                         unsigned int* ticket) {
+    if (SHARED_P) {
+        if (!active) {
+#pragma unroll
+            for (int q = 0; q < P; q++) acc[q] = 0.0;
+        }
+        reduce_dp<P>(acc, partials, dp, ticket);
+    } else if (active) {
+#pragma unroll
+        for (int q = 0; q < P; q++) dp_members[(int64_t)q * N + i] = acc[q];
+    }
+}
+
+// Body of the three QuadratureAdjoint kernels (tsit5_quad.cuh, tsit5_adaptive.cuh, ros23.cuh), which differ only in `make(i)`,
+// member i's integrand context: quad_member_loop over the members, per-member dp stored as each member finishes, a shared p
+// summed over the grid (lane 0 of each warp carries its members' sum).  Here rather than next to quad_member_loop because
+// quadgk.cuh comes before reduce_dp.
+template <int P, bool SHARED_P, class Args, class MAKE>
+__device__ __forceinline__ void quad_kernel_body(const Args& a, const MAKE& make) {
+    extern __shared__ double s_quad_l1[];
+    const int lane = threadIdx.x & 31;
+    double acc[P];
+#pragma unroll
+    for (int q = 0; q < P; q++) acc[q] = 0.0;
+    auto sink = [&](int64_t i, const double* res) {
+        if (SHARED_P) {
+#pragma unroll
+            for (int q = 0; q < P; q++) acc[q] += res[q];
+        } else if (lane == 0) {
+#pragma unroll
+            for (int q = 0; q < P; q++) a.dp_members[(int64_t)q * a.N + i] = res[q];
+        }
+    };
+    quad_member_loop<P>(a.N, a.K, a.saveat, a.t0, a.t1, a.quad_abstol, a.quad_reltol, a.qseg, a.qkey, a.maxseg, s_quad_l1, make, sink);
+    if (SHARED_P) store_dp<P, true>(acc, lane == 0, 0, a.N, a.dp_members, a.partials, a.dp, a.ticket);
+}
+
 // accumulate_cost! (src/derivative_wrappers.jl:1411-1442): with ka' = -dlam/dt the continuous cost adds +dgdu_continuous(y)
 template <int D, bool CONT, class Args, class R>
 __device__ __forceinline__ void add_continuous(const Args& a, const R* y, R* ka) {
@@ -756,6 +797,7 @@ __global__ void __maxnreg__(B200_REV_MAXREG) tsit5_reverse_kernel(const __grid_c
         asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
         a.trace[blockIdx.x * 3 + 2] = t;
     }
+    // written out here rather than through store_dp, which reorders this kernel's instructions at the same register count
     if (SHARED_P) {
         if (!active) {
 #pragma unroll

@@ -163,6 +163,43 @@ struct FwdDense {
     }
 };
 
+// ---- one Rosenbrock23 step of z' = rhs(t, z) over [t, t + hs] with hd = hs d, f0 = rhs(t, z) and W factored by the caller
+// (solveW(b): b <- W^-1 b): the stages k1, k2, the new state zn, fnr = rhs(t + hs, zn) (FSAL) and the error estimate.
+// HAS_DT: non-autonomous rhs, the stages carry hd dT with dT = d rhs/dt at (t, z).  (A template flag rather than a zero dT:
+// f0 + hd 0 would turn -0 into +0.)
+template <int L, bool HAS_DT, class RHS, class SOLVEW>
+__device__ __forceinline__ double ros23_step(const RosArgs& a, const RHS& rhs, const SOLVEW& solveW, double t, double hs, double hd,
+                                             const double* z, const double* f0, const double* dT, double* k1, double* k2,
+                                             double* zn, double* fnr) {
+    double k3[L], f1[L], tmp[L];
+#pragma unroll
+    for (int c = 0; c < L; c++) k1[c] = HAS_DT ? f0[c] + hd * dT[c] : f0[c];
+    solveW(k1);
+#pragma unroll
+    for (int c = 0; c < L; c++) tmp[c] = z[c] + 0.5 * hs * k1[c];
+    rhs(t + 0.5 * hs, tmp, f1);
+#pragma unroll
+    for (int c = 0; c < L; c++) k2[c] = f1[c] - k1[c];
+    solveW(k2);
+#pragma unroll
+    for (int c = 0; c < L; c++) { k2[c] += k1[c]; zn[c] = z[c] + hs * k2[c]; }
+    rhs(t + hs, zn, fnr);
+#pragma unroll
+    for (int c = 0; c < L; c++) {
+        k3[c] = fnr[c] - ROS_E32 * (k2[c] - f1[c]) - 2 * (k1[c] - f0[c]);
+        if (HAS_DT) k3[c] += hd * dT[c];
+    }
+    solveW(k3);
+    double e2 = 0;
+#pragma unroll
+    for (int c = 0; c < L; c++) {
+        const double e = hs / 6.0 * (k1[c] - 2 * k2[c] + k3[c]);
+        const double sc = a.abstol + a.reltol * fmax(fabs(z[c]), fabs(zn[c]));
+        e2 += (e / sc) * (e / sc);
+    }
+    return sqrt(e2 / L);
+}
+
 // ------------------------------------------------------------------------------------------------------------
 template <class Fam, bool SHARED_P>
 __global__ void __launch_bounds__(256) ros23_forward_kernel(RosArgs a) {
@@ -173,8 +210,10 @@ __global__ void __launch_bounds__(256) ros23_forward_kernel(RosArgs a) {
     double p[P];
 #pragma unroll
     for (int q = 0; q < P; q++) p[q] = SHARED_P ? a.p[q] : a.p[(int64_t)q * N + i];
-    double u[D], f0[D], k1[D], k2[D], k3[D], f1[D], un[D], fn[D], tmp[D], err[D], W[D][D];
+    double u[D], f0[D], k1[D], k2[D], un[D], fn[D], W[D][D];
     int piv[D];
+    auto rhs = [&](double, const double* x, double* dx) { Fam::f(x, p, dx); };
+    auto solveW = [&](double* b) { lu_solve<D>(W, piv, b); };
 #pragma unroll
     for (int j = 0; j < D; j++) { u[j] = a.u0[(int64_t)j * N + i]; a.fu[(int64_t)j * N + i] = u[j]; }
     a.ft[i] = a.t0;
@@ -199,29 +238,7 @@ __global__ void __launch_bounds__(256) ros23_forward_kernel(RosArgs a) {
 #pragma unroll
             for (int c = 0; c < D; c++) W[r][c] = (r == c ? 1.0 : 0.0) - h * ROS_D * W[r][c];
         if (!lu_factor<D>(W, piv)) { stat = 1; break; }
-#pragma unroll
-        for (int j = 0; j < D; j++) k1[j] = f0[j];
-        lu_solve<D>(W, piv, k1);
-#pragma unroll
-        for (int j = 0; j < D; j++) tmp[j] = u[j] + 0.5 * h * k1[j];
-        Fam::f(tmp, p, f1);
-#pragma unroll
-        for (int j = 0; j < D; j++) k2[j] = f1[j] - k1[j];
-        lu_solve<D>(W, piv, k2);
-#pragma unroll
-        for (int j = 0; j < D; j++) { k2[j] += k1[j]; un[j] = u[j] + h * k2[j]; }
-        Fam::f(un, p, fn);
-#pragma unroll
-        for (int j = 0; j < D; j++) k3[j] = fn[j] - ROS_E32 * (k2[j] - f1[j]) - 2 * (k1[j] - f0[j]);
-        lu_solve<D>(W, piv, k3);
-        double e2 = 0;
-#pragma unroll
-        for (int j = 0; j < D; j++) {
-            err[j] = h / 6.0 * (k1[j] - 2 * k2[j] + k3[j]);
-            const double sc = a.abstol + a.reltol * fmax(fabs(u[j]), fabs(un[j]));
-            e2 += (err[j] / sc) * (err[j] / sc);
-        }
-        const double EEst = sqrt(e2 / D);
+        const double EEst = ros23_step<D, false>(a, rhs, solveW, t, h, 0.0, u, f0, nullptr, k1, k2, un, fn);
         const double q = step_factor_I(EEst);
         if (EEst <= 1.0) {
             const double tn = last ? a.t1 : t + h;
@@ -253,19 +270,24 @@ __global__ void __launch_bounds__(256) ros23_forward_kernel(RosArgs a) {
     if (a.status) a.status[i] = stat;
 }
 
-// adjoint RHS  dlam = -J(y(t))' lam  (right-continuous forward lookup) and, on request, its Jacobian / time derivative
-template <class Fam, int D>
-__device__ __forceinline__ void adj_rhs(const FwdDense<D>& sol, const double* p, double t, const double* lam, double* out) {
-    double y[D];
-    sol.eval(t, true, y, nullptr);
-    Fam::vjp_u(y, p, lam, out);
-#pragma unroll
-    for (int j = 0; j < D; j++) out[j] = -out[j];
-}
-
+// ------------------------------------------------------------------------------------------------------------
+// Reverse adjoint solve.  SA_GAUSS / SA_GK / SA_QUAD: z = lam (L = D); SA_INTERP: z = [lam; mu] (L = D + P); SA_BACKSOLVE:
+// z = [lam; mu; y] (L = 2D + P), y integrated backwards and reset from the forward solution at the checkpoints
+// (src/interpolating_adjoint.jl:150-174, src/backsolve_adjoint.jl:32-61; the reference runs every sensealg with stiff solvers,
+// test/Core2/stiff_adjoints.jl:204-252).  W = I - h d (d rhs / dz) is block triangular, so the linear solves are the D x D LU
+// of the lambda block (and of the y block for Backsolve) plus substitutions:
+//   lambda only     W = I + hd J'                                                    dT = -(dJ/dt)'lam   (ydot from sol)
+//   Interpolating   W = [[I + hd J', 0], [hd F', I]]                                 dT = [-(dJ/dt)'lam, -(dF/dt)'lam]
+//   Backsolve       W = [[I + hd J', 0, hd H], [hd F', I, hd G], [0, 0, I - hd J]]   autonomous: dT = 0
+//                   H v = d(J'lam)/dy [v], G v = d(F'lam)/dy [v]  (families.cuh::djac, dvjp_p)
+// Error norm over all components of z (the reference's state).  Checkpoints / jumps as in t5a_reverse_kernel.  A singular W,
+// a non-finite error estimate, the iteration cap or a full QuadratureAdjoint record fail the member loudly: NaN du0 and dp
+// (rn = -1), never a silent partial.
+// ------------------------------------------------------------------------------------------------------------
 template <class Fam, int SA, bool SHARED_P, int COST>
 __global__ void __launch_bounds__(256) ros23_reverse_kernel(RosArgs a) {
-    constexpr int D = Fam::D, P = Fam::P;
+    constexpr int D = Fam::D, P = Fam::P, L = (SA == SA_INTERP) ? D + P : (SA == SA_BACKSOLVE ? 2 * D + P : D);
+    constexpr int YO = (SA == SA_BACKSOLVE) ? D + P : 0;          // offset of y inside z (Backsolve)
     const int64_t gi = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     const bool active = gi < a.N;
     const int64_t i = active ? gi : a.N - 1;
@@ -275,184 +297,31 @@ __global__ void __launch_bounds__(256) ros23_reverse_kernel(RosArgs a) {
     for (int q = 0; q < P; q++) { p[q] = SHARED_P ? a.p[q] : a.p[(int64_t)q * N + i]; acc[q] = 0.0; }
     FwdDense<D> sol{a.ft, a.fu, a.fk, N, i, a.fn[i]};
     sol.cur = sol.n - 1;                  // the reverse solve starts at T
-    double z[D], zn[D], f0[D], k1[D], k2[D], k3[D], f1[D], fnr[D], tmp[D], W[D][D], dT[D];
-    int piv[D];
-#pragma unroll
-    for (int j = 0; j < D; j++) z[j] = 0.0;
-    const double T = a.t1, t0 = a.t0;
-    double t = T;
-    int cur = a.K - 1, nrev = 0;
-    bool fsal_ok = false, overflow = false;
-    auto jump_if_at = [&](double tt) {
-        while (cur >= 0 && fabs(a.saveat[cur] - tt) <= EPS100 * fmax(fabs(tt), 1.0)) {
-            if (!((a.flags & KF_NO_START) && cur == 0)) {
-                double y[D];
-                if (COST == COST_EXPLICIT) {
-#pragma unroll
-                    for (int j = 0; j < D; j++) z[j] += a.dLdu[((int64_t)cur * D + j) * N + i];
-                } else {
-                    sol.eval(a.saveat[cur], true, y, nullptr);
-#pragma unroll
-                    for (int j = 0; j < D; j++) z[j] += a.cost_a[j] * y[j] + a.cost_b[j];
-                }
-            }
-            cur--; fsal_ok = false;
-        }
-    };
-    jump_if_at(t);
-    double h = -1e-4 * (T - t0);
-    long iters = 0;
-    while (t > t0 && sol.n > 0) {
-        if (++iters > 50000000L || (SA == SA_QUAD && nrev >= a.maxs)) { overflow = true; break; }
-        double tstop = t0;
-        if (cur >= 0 && a.saveat[cur] < t && a.saveat[cur] > tstop) tstop = a.saveat[cur];
-        double tn = tstop_snap(t + h, tstop);
-        if (tn < tstop) tn = tstop;
-        const double hs = tn - t;
-        if (!fsal_ok) adj_rhs<Fam, D>(sol, p, t, z, f0);
-        // Jacobian of the adjoint RHS wrt lambda (-J') and its time derivative -(dJ/dt)' lambda, ydot from the interpolant
-        {
-            double y[D], yd[D], J[D][D], dJ[D][D];
-            sol.eval(t, true, y, yd);
-            Fam::jac(y, p, J); Fam::djac(p, yd, dJ);
-#pragma unroll
-            for (int r = 0; r < D; r++) {
-                double s = 0;
-#pragma unroll
-                for (int c = 0; c < D; c++) { W[r][c] = (r == c ? 1.0 : 0.0) - hs * ROS_D * (-J[c][r]); s -= dJ[c][r] * z[c]; }
-                dT[r] = s;
-            }
-        }
-        if (!lu_factor<D>(W, piv)) break;
-#pragma unroll
-        for (int j = 0; j < D; j++) k1[j] = f0[j] + hs * ROS_D * dT[j];
-        lu_solve<D>(W, piv, k1);
-#pragma unroll
-        for (int j = 0; j < D; j++) tmp[j] = z[j] + 0.5 * hs * k1[j];
-        adj_rhs<Fam, D>(sol, p, t + 0.5 * hs, tmp, f1);
-#pragma unroll
-        for (int j = 0; j < D; j++) k2[j] = f1[j] - k1[j];
-        lu_solve<D>(W, piv, k2);
-#pragma unroll
-        for (int j = 0; j < D; j++) { k2[j] += k1[j]; zn[j] = z[j] + hs * k2[j]; }
-        adj_rhs<Fam, D>(sol, p, t + hs, zn, fnr);
-#pragma unroll
-        for (int j = 0; j < D; j++) k3[j] = fnr[j] - ROS_E32 * (k2[j] - f1[j]) - 2 * (k1[j] - f0[j]) + hs * ROS_D * dT[j];
-        lu_solve<D>(W, piv, k3);
-        double e2 = 0;
-#pragma unroll
-        for (int j = 0; j < D; j++) {
-            const double e = hs / 6.0 * (k1[j] - 2 * k2[j] + k3[j]);
-            const double sc = a.abstol + a.reltol * fmax(fabs(z[j]), fabs(zn[j]));
-            e2 += (e / sc) * (e / sc);
-        }
-        const double EEst = sqrt(e2 / D);
-        const double q = step_factor_I(EEst);
-        if (EEst > 1.0) { h = hs / q; fsal_ok = true; continue; }
-        h = hs / q;
-        if (SA == SA_GAUSS) {
-            // IntegratingSumCallback, n = (alg_order+1) div 2 = 1 node: midpoint, weight 2, scale (tn - t)/2, integrand -F'lam
-            const double tj = 0.5 * (tn + t), th = (tj - t) / hs;
-            const double c1 = th * (1 - th) / (1 - 2 * ROS_D), c2 = th * (th - 2 * ROS_D) / (1 - 2 * ROS_D);
-            double lq[D], y[D], dg[P];
-#pragma unroll
-            for (int j = 0; j < D; j++) lq[j] = z[j] + hs * (c1 * k1[j] + c2 * k2[j]);
-            sol.eval(tj, false, y, nullptr);
-            Fam::vjp_p(y, p, lq, dg);
-#pragma unroll
-            for (int q2 = 0; q2 < P; q2++) acc[q2] += (0.5 * (tn - t)) * 2.0 * (-dg[q2]);
-        } else if (SA == SA_GK) {
-            auto node = [&](double tj, double* out) {
-                const double th = (tj - t) / hs;
-                const double c1 = th * (1 - th) / (1 - 2 * ROS_D), c2 = th * (th - 2 * ROS_D) / (1 - 2 * ROS_D);
-                double lq[D], y[D];
-#pragma unroll
-                for (int j = 0; j < D; j++) lq[j] = z[j] + hs * (c1 * k1[j] + c2 * k2[j]);
-                sol.eval(tj, false, y, nullptr);
-                Fam::vjp_p(y, p, lq, out);
-#pragma unroll
-                for (int q2 = 0; q2 < P; q2++) out[q2] = -out[q2];
-            };
-            integrate_gk_step<P, 1>(node, t, tn, acc);
-        } else if (active) {
-            double* rec = a.rrec + ((int64_t)i * a.maxs + nrev) * quad_pad(3 + 3 * D);
-            rec[0] = t; rec[1] = hs; rec[2 + 3 * D] = 1.0 / hs;
-            a.rend[(int64_t)i * a.maxs + nrev] = t + hs;
-#pragma unroll
-            for (int j = 0; j < D; j++) { rec[2 + j] = z[j]; rec[2 + D + j] = k1[j]; rec[2 + 2 * D + j] = k2[j]; }
-        }
-        nrev++;
-#pragma unroll
-        for (int j = 0; j < D; j++) { z[j] = zn[j]; f0[j] = fnr[j]; }
-        fsal_ok = true;
-        t = tn;
-        jump_if_at(t);
-    }
-    if (active) {
-        // a member whose dense reverse solution did not fit (max steps) fails loudly: NaN gradient, never a silent partial
-#pragma unroll
-        for (int j = 0; j < D; j++) a.du0[(int64_t)j * N + i] = overflow ? __longlong_as_double(0x7ff8000000000000LL) : z[j];
-        if (SA == SA_QUAD) a.rn[i] = overflow ? -1 : nrev;
-    }
-    if (SA == SA_GAUSS || SA == SA_GK) {
-        if (SHARED_P) {
-            if (!active) {
-#pragma unroll
-                for (int q = 0; q < P; q++) acc[q] = 0.0;
-            }
-            reduce_dp<P>(acc, a.partials, a.dp, a.ticket);
-        } else if (active) {
-#pragma unroll
-            for (int q = 0; q < P; q++) a.dp_members[(int64_t)q * N + i] = acc[q];
-        }
-    }
-}
-
-// ------------------------------------------------------------------------------------------------------------
-// Rosenbrock23 on the AUGMENTED adjoint states: InterpolatingAdjoint z = [lam; mu] and BacksolveAdjoint z = [lam; mu; y]
-// (src/interpolating_adjoint.jl:150-174, src/backsolve_adjoint.jl:32-61; the reference runs every sensealg with stiff solvers,
-// test/Core2/stiff_adjoints.jl:204-252).  W = I - h d (d rhs / dz) is block triangular, so the linear solves are the 3 x 3 LU
-// of the lambda block (and of the y block for Backsolve) plus substitutions:
-//   Interpolating   W = [[I + hd J', 0], [hd F', I]]                         dT = [-(dJ/dt)'lam, -(dF/dt)'lam]   (ydot from sol)
-//   Backsolve       W = [[I + hd J', 0, hd H], [hd F', I, hd G], [0, 0, I - hd J]]   autonomous: dT = 0
-//                   H v = d(J'lam)/dy [v], G v = d(F'lam)/dy [v]  (families.cuh::djac, dvjp_p)
-// Error norm over all components of z (the reference's augmented state).  Checkpoints / jumps as in t5a_reverse_kernel.
-// ------------------------------------------------------------------------------------------------------------
-template <class Fam, int SA, bool SHARED_P, int COST>
-__global__ void __launch_bounds__(256) ros23_aug_reverse_kernel(RosArgs a) {
-    static_assert(SA == SA_INTERP || SA == SA_BACKSOLVE, "augmented states only");
-    constexpr int D = Fam::D, P = Fam::P, L = (SA == SA_INTERP) ? D + P : 2 * D + P, YO = D + P;
-    const int64_t gi = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    const bool active = gi < a.N;
-    const int64_t i = active ? gi : a.N - 1;
-    const int64_t N = a.N;
-    double p[P];
-#pragma unroll
-    for (int q = 0; q < P; q++) p[q] = SHARED_P ? a.p[q] : a.p[(int64_t)q * N + i];
-    FwdDense<D> sol{a.ft, a.fu, a.fk, N, i, a.fn[i]};
-    sol.cur = sol.n - 1;
-    double z[L], zn[L], f0[L], k1[L], k2[L], k3[L], f1[L], fnr[L], tmp[L], dT[L];
+    double z[L], zn[L], f0[L], k1[L], k2[L], fnr[L], dT[L];
     double Wl[D][D], Wy[D][D], yj[D], lamj[D];            // Jacobian point of the current step (y, lam at t)
     int pivl[D], pivy[D];
 #pragma unroll
     for (int c = 0; c < L; c++) { z[c] = 0.0; dT[c] = 0.0; }
+    // adjoint RHS: dlam = -J(y(t))' lam, dmu = -F(y(t))' lam  (right-continuous forward lookup), dy = f(y)
     auto rhs = [&](double tt, const double* x, double* dx) {
-        double y[D], dg[P];
+        double y[D];
         if (SA == SA_BACKSOLVE) {
 #pragma unroll
             for (int j = 0; j < D; j++) y[j] = x[YO + j];
         } else sol.eval(tt, true, y, nullptr);
         Fam::vjp_u(y, p, x, dx);
-        Fam::vjp_p(y, p, x, dg);
 #pragma unroll
         for (int j = 0; j < D; j++) dx[j] = -dx[j];
+        if (L > D) {
+            double dg[P];
+            Fam::vjp_p(y, p, x, dg);
 #pragma unroll
-        for (int q = 0; q < P; q++) dx[D + q] = -dg[q];
+            for (int q = 0; q < P; q++) dx[D + q] = -dg[q];
+        }
         if (SA == SA_BACKSOLVE) Fam::f(y, p, dx + YO);
     };
     double hd = 0.0;                                     // hs * d of the current step
     auto solveW = [&](double* b) {
-        double dg[P];
         if (SA == SA_BACKSOLVE) {
             lu_solve<D>(Wy, pivy, b + YO);
             double dJ[D][D];
@@ -466,18 +335,21 @@ __global__ void __launch_bounds__(256) ros23_aug_reverse_kernel(RosArgs a) {
             }
         }
         lu_solve<D>(Wl, pivl, b);
-        Fam::vjp_p(yj, p, b, dg);
-#pragma unroll
-        for (int q = 0; q < P; q++) b[D + q] -= hd * dg[q];
-        if (SA == SA_BACKSOLVE) {
-            Fam::dvjp_p(yj, p, b + YO, lamj, dg);
+        if (L > D) {
+            double dg[P];
+            Fam::vjp_p(yj, p, b, dg);
 #pragma unroll
             for (int q = 0; q < P; q++) b[D + q] -= hd * dg[q];
+            if (SA == SA_BACKSOLVE) {
+                Fam::dvjp_p(yj, p, b + YO, lamj, dg);
+#pragma unroll
+                for (int q = 0; q < P; q++) b[D + q] -= hd * dg[q];
+            }
         }
     };
     const double T = a.t1, t0 = a.t0;
     double t = T;
-    int cur = a.K - 1, ck = sol.n;
+    int cur = a.K - 1, ck = sol.n, nrev = 0;
     bool fsal_ok = false, failed = false;
     const bool ckpt_on = !(a.flags & KF_NO_CHECKPOINTING), every = (a.flags & KF_CKPT_EVERY_STEP);
     if (SA == SA_BACKSOLVE) {
@@ -526,7 +398,7 @@ __global__ void __launch_bounds__(256) ros23_aug_reverse_kernel(RosArgs a) {
     double h = -1e-4 * (T - t0);
     long iters = 0;
     while (t > t0 && sol.n > 0) {
-        if (++iters > 50000000L) { failed = true; break; }
+        if (++iters > 50000000L || (SA == SA_QUAD && nrev >= a.maxs)) { failed = true; break; }
         double tstop = t0;
         if (cur >= 0 && a.saveat[cur] < t && a.saveat[cur] > tstop) tstop = a.saveat[cur];
         if (SA == SA_BACKSOLVE && ckpt_on && every) {            // every forward knot is a tstop of the reverse solve
@@ -540,10 +412,10 @@ __global__ void __launch_bounds__(256) ros23_aug_reverse_kernel(RosArgs a) {
         hd = hs * ROS_D;
         if (!fsal_ok) rhs(t, z, f0);
         {   // Jacobian blocks and the time derivative at (t, z)
-            double yd[D], J[D][D], dJ[D][D], dg[P];
+            double yd[D], J[D][D];
             if (SA == SA_BACKSOLVE) {
 #pragma unroll
-                for (int j = 0; j < D; j++) { yj[j] = z[YO + j]; yd[j] = 0.0; }
+                for (int j = 0; j < D; j++) yj[j] = z[YO + j];
             } else sol.eval(t, true, yj, yd);
 #pragma unroll
             for (int j = 0; j < D; j++) lamj[j] = z[j];
@@ -551,10 +423,13 @@ __global__ void __launch_bounds__(256) ros23_aug_reverse_kernel(RosArgs a) {
 #pragma unroll
             for (int r = 0; r < D; r++)
 #pragma unroll
-                for (int c = 0; c < D; c++) { Wl[r][c] = (r == c ? 1.0 : 0.0) + hd * J[c][r]; Wy[r][c] = (r == c ? 1.0 : 0.0) - hd * J[r][c]; }
-            if (SA == SA_INTERP) {
+                for (int c = 0; c < D; c++) {
+                    Wl[r][c] = (r == c ? 1.0 : 0.0) + hd * J[c][r];
+                    if (SA == SA_BACKSOLVE) Wy[r][c] = (r == c ? 1.0 : 0.0) - hd * J[r][c];
+                }
+            if (SA != SA_BACKSOLVE) {
+                double dJ[D][D];
                 Fam::djac(p, yd, dJ);
-                Fam::dvjp_p(yj, p, yd, lamj, dg);
 #pragma unroll
                 for (int r = 0; r < D; r++) {
                     double s = 0;
@@ -562,38 +437,52 @@ __global__ void __launch_bounds__(256) ros23_aug_reverse_kernel(RosArgs a) {
                     for (int c = 0; c < D; c++) s -= dJ[c][r] * lamj[c];
                     dT[r] = s;
                 }
+            }
+            if (SA == SA_INTERP) {
+                double dg[P];
+                Fam::dvjp_p(yj, p, yd, lamj, dg);
 #pragma unroll
                 for (int q = 0; q < P; q++) dT[D + q] = -dg[q];
             }
         }
         if (!lu_factor<D>(Wl, pivl) || (SA == SA_BACKSOLVE && !lu_factor<D>(Wy, pivy))) { failed = true; break; }
-#pragma unroll
-        for (int c = 0; c < L; c++) k1[c] = f0[c] + hd * dT[c];
-        solveW(k1);
-#pragma unroll
-        for (int c = 0; c < L; c++) tmp[c] = z[c] + 0.5 * hs * k1[c];
-        rhs(t + 0.5 * hs, tmp, f1);
-#pragma unroll
-        for (int c = 0; c < L; c++) k2[c] = f1[c] - k1[c];
-        solveW(k2);
-#pragma unroll
-        for (int c = 0; c < L; c++) { k2[c] += k1[c]; zn[c] = z[c] + hs * k2[c]; }
-        rhs(t + hs, zn, fnr);
-#pragma unroll
-        for (int c = 0; c < L; c++) k3[c] = fnr[c] - ROS_E32 * (k2[c] - f1[c]) - 2 * (k1[c] - f0[c]) + hd * dT[c];
-        solveW(k3);
-        double e2 = 0;
-#pragma unroll
-        for (int c = 0; c < L; c++) {
-            const double e = hs / 6.0 * (k1[c] - 2 * k2[c] + k3[c]);
-            const double sc = a.abstol + a.reltol * fmax(fabs(z[c]), fabs(zn[c]));
-            e2 += (e / sc) * (e / sc);
-        }
-        const double EEst = sqrt(e2 / L);
+        const double EEst = ros23_step<L, true>(a, rhs, solveW, t, hs, hd, z, f0, dT, k1, k2, zn, fnr);
         if (!isfinite(EEst)) { failed = true; break; }           // e.g. Backsolve blowing up backwards on a stiff problem
         const double q = step_factor_I(EEst);
         if (EEst > 1.0) { h = hs / q; fsal_ok = true; continue; }
         h = hs / q;
+        if (SA == SA_GAUSS) {
+            // IntegratingSumCallback, n = (alg_order+1) div 2 = 1 node: midpoint, weight 2, scale (tn - t)/2, integrand -F'lam
+            const double tj = 0.5 * (tn + t), th = (tj - t) / hs;
+            const double c1 = th * (1 - th) / (1 - 2 * ROS_D), c2 = th * (th - 2 * ROS_D) / (1 - 2 * ROS_D);
+            double lq[D], y[D], dg[P];
+#pragma unroll
+            for (int j = 0; j < D; j++) lq[j] = z[j] + hs * (c1 * k1[j] + c2 * k2[j]);
+            sol.eval(tj, false, y, nullptr);
+            Fam::vjp_p(y, p, lq, dg);
+#pragma unroll
+            for (int q2 = 0; q2 < P; q2++) acc[q2] += (0.5 * (tn - t)) * 2.0 * (-dg[q2]);
+        } else if (SA == SA_GK) {
+            auto node = [&](double tj, double* out) {
+                const double th = (tj - t) / hs;
+                const double c1 = th * (1 - th) / (1 - 2 * ROS_D), c2 = th * (th - 2 * ROS_D) / (1 - 2 * ROS_D);
+                double lq[D], y[D];
+#pragma unroll
+                for (int j = 0; j < D; j++) lq[j] = z[j] + hs * (c1 * k1[j] + c2 * k2[j]);
+                sol.eval(tj, false, y, nullptr);
+                Fam::vjp_p(y, p, lq, out);
+#pragma unroll
+                for (int q2 = 0; q2 < P; q2++) out[q2] = -out[q2];
+            };
+            integrate_gk_step<P, 1>(node, t, tn, acc);
+        } else if (SA == SA_QUAD && active) {
+            double* rec = a.rrec + ((int64_t)i * a.maxs + nrev) * quad_pad(3 + 3 * D);
+            rec[0] = t; rec[1] = hs; rec[2 + 3 * D] = 1.0 / hs;
+            a.rend[(int64_t)i * a.maxs + nrev] = t + hs;
+#pragma unroll
+            for (int j = 0; j < D; j++) { rec[2 + j] = z[j]; rec[2 + D + j] = k1[j]; rec[2 + 2 * D + j] = k2[j]; }
+        }
+        nrev++;
 #pragma unroll
         for (int c = 0; c < L; c++) { z[c] = zn[c]; f0[c] = fnr[c]; }
         fsal_ok = true;
@@ -605,19 +494,13 @@ __global__ void __launch_bounds__(256) ros23_aug_reverse_kernel(RosArgs a) {
     if (active) {
 #pragma unroll
         for (int j = 0; j < D; j++) a.du0[(int64_t)j * N + i] = failed ? qnan : z[j];
+        if (SA == SA_QUAD) a.rn[i] = failed ? -1 : nrev;
     }
-    double out[P];
+    if (SA != SA_QUAD) {
+        double out[P];
 #pragma unroll
-    for (int q = 0; q < P; q++) out[q] = failed ? qnan : z[D + q];
-    if (SHARED_P) {
-        if (!active) {
-#pragma unroll
-            for (int q = 0; q < P; q++) out[q] = 0.0;
-        }
-        reduce_dp<P>(out, a.partials, a.dp, a.ticket);
-    } else if (active) {
-#pragma unroll
-        for (int q = 0; q < P; q++) a.dp_members[(int64_t)q * N + i] = out[q];
+        for (int q = 0; q < P; q++) out[q] = failed ? qnan : (L > D ? z[(L > D ? D : 0) + (L > D ? q : 0)] : acc[q]);
+        store_dp<P, SHARED_P>(out, active, i, N, a.dp_members, a.partials, a.dp, a.ticket);
     }
 }
 
@@ -663,36 +546,13 @@ struct RosQuadCtx {
 template <class Fam, bool SHARED_P>
 __global__ void __launch_bounds__(QUAD_WARPS * 32) ros23_quadrature_kernel(RosArgs a) {
     constexpr int D = Fam::D, P = Fam::P;
-    extern __shared__ double s_quad_l1[];
-    const int lane = threadIdx.x & 31;
-    const int64_t N = a.N;
-    double acc[P];
-#pragma unroll
-    for (int q = 0; q < P; q++) acc[q] = 0.0;
-    auto make = [&](int64_t i) {
+    quad_kernel_body<P, SHARED_P>(a, [&](int64_t i) {
         RosQuadCtx<Fam, D, P> c{a.ftT + (int64_t)i * (a.maxs + 1), a.frecT + (int64_t)i * a.maxs * quad_pad(3 * D + 3),
                                 a.rrec + (int64_t)i * a.maxs * quad_pad(3 + 3 * D), a.rend + (int64_t)i * a.maxs, a.fn[i], a.rn[i], {}};
 #pragma unroll
-        for (int q = 0; q < P; q++) c.p[q] = SHARED_P ? a.p[q] : a.p[(int64_t)q * N + i];
+        for (int q = 0; q < P; q++) c.p[q] = SHARED_P ? a.p[q] : a.p[(int64_t)q * a.N + i];
         return c;
-    };
-    auto sink = [&](int64_t i, const double* res) {
-        if (SHARED_P) {
-#pragma unroll
-            for (int q = 0; q < P; q++) acc[q] += res[q];
-        } else if (lane == 0) {
-#pragma unroll
-            for (int q = 0; q < P; q++) a.dp_members[(int64_t)q * N + i] = res[q];
-        }
-    };
-    quad_member_loop<P>(N, a.K, a.saveat, a.t0, a.t1, a.quad_abstol, a.quad_reltol, a.qseg, a.qkey, a.maxseg, s_quad_l1, make, sink);
-    if (SHARED_P) {
-        if (lane != 0) {
-#pragma unroll
-            for (int q = 0; q < P; q++) acc[q] = 0.0;
-        }
-        reduce_dp<P>(acc, a.partials, a.dp, a.ticket);
-    }
+    });
 }
 
 }  // namespace b200adj

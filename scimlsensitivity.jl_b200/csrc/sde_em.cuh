@@ -209,16 +209,7 @@ __global__ void __launch_bounds__(512) sde_backsolve_kernel(SdeRevArgs a) {
         }
     }
     if (active) store_state<D>(a.du0, N, i, lam);
-    if (SHARED_P) {
-        if (!active) {
-#pragma unroll
-            for (int q = 0; q < P; q++) mu[q] = 0.0;
-        }
-        reduce_dp<P>(mu, a.partials, a.dp, a.ticket);
-    } else if (active) {
-#pragma unroll
-        for (int q = 0; q < P; q++) a.dp_members[(int64_t)q * N + i] = mu[q];
-    }
+    store_dp<P, SHARED_P>(mu, active, i, N, a.dp_members, a.partials, a.dp, a.ticket);
 }
 
 }  // namespace b200adj

@@ -901,16 +901,7 @@ __global__ void __launch_bounds__(256) t5a_reverse_kernel(const __grid_constant_
         double out[P];
 #pragma unroll
         for (int q = 0; q < P; q++) out[q] = overflow ? qnan : ((SA == SA_INTERP || SA == SA_BACKSOLVE) ? z[(L > D ? D : 0) + (L > D ? q : 0)] : acc[q]);
-        if (SHARED_P) {
-            if (!active) {
-#pragma unroll
-                for (int q = 0; q < P; q++) out[q] = 0.0;
-            }
-            reduce_dp<P>(out, a.partials, a.dp, a.ticket);
-        } else if (active) {
-#pragma unroll
-            for (int q = 0; q < P; q++) a.dp_members[(int64_t)q * N + i] = out[q];
-        }
+        store_dp<P, SHARED_P>(out, active, i, N, a.dp_members, a.partials, a.dp, a.ticket);
     }
 }
 
@@ -955,36 +946,13 @@ struct T5aQuadCtx {
 template <class Fam, bool SHARED_P>
 __global__ void __launch_bounds__(QUAD_WARPS * 32) t5a_quadrature_kernel(const __grid_constant__ T5aArgs a) {
     constexpr int D = Fam::D, P = Fam::P;
-    extern __shared__ double s_quad_l1[];
-    const int lane = threadIdx.x & 31;
-    const int64_t N = a.N;
-    double acc[P];
-#pragma unroll
-    for (int q = 0; q < P; q++) acc[q] = 0.0;
-    auto make = [&](int64_t i) {
+    quad_kernel_body<P, SHARED_P>(a, [&](int64_t i) {
         T5aQuadCtx<Fam, D, P> c{a, a.ftT + (int64_t)i * (a.maxs + 1), a.frecT + (int64_t)i * (a.maxs + 1) * t5_rec<D>(),
                                 a.rrec + (int64_t)i * a.maxs * quad_pad(3 + 8 * D), a.rend + (int64_t)i * a.maxs, a.fn[i], a.rn[i], {}};
 #pragma unroll
-        for (int q = 0; q < P; q++) c.p[q] = SHARED_P ? a.p[q] : a.p[(int64_t)q * N + i];
+        for (int q = 0; q < P; q++) c.p[q] = SHARED_P ? a.p[q] : a.p[(int64_t)q * a.N + i];
         return c;
-    };
-    auto sink = [&](int64_t i, const double* res) {
-        if (SHARED_P) {
-#pragma unroll
-            for (int q = 0; q < P; q++) acc[q] += res[q];
-        } else if (lane == 0) {
-#pragma unroll
-            for (int q = 0; q < P; q++) a.dp_members[(int64_t)q * N + i] = res[q];
-        }
-    };
-    quad_member_loop<P>(N, a.K, a.saveat, a.t0, a.t1, a.quad_abstol, a.quad_reltol, a.qseg, a.qkey, a.maxseg, s_quad_l1, make, sink);
-    if (SHARED_P) {
-        if (lane != 0) {
-#pragma unroll
-            for (int q = 0; q < P; q++) acc[q] = 0.0;
-        }
-        reduce_dp<P>(acc, a.partials, a.dp, a.ticket);
-    }
+    });
 }
 
 }  // namespace b200adj

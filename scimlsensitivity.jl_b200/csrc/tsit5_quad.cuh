@@ -67,35 +67,12 @@ struct Tsit5QuadCtx {
 template <class Fam, bool SHARED_P>
 __global__ void __launch_bounds__(QUAD_WARPS * 32) tsit5_quadrature_kernel(const __grid_constant__ Tsit5QuadArgs a) {
     constexpr int D = Fam::D, P = Fam::P;
-    extern __shared__ double s_quad_l1[];
-    const int lane = threadIdx.x & 31;
-    const int64_t N = a.N;
-    double acc[P];
-#pragma unroll
-    for (int q = 0; q < P; q++) acc[q] = 0.0;
-    auto make = [&](int64_t i) {
+    quad_kernel_body<P, SHARED_P>(a, [&](int64_t i) {
         Tsit5QuadCtx<Fam, D, P> c{a, i, {}};
 #pragma unroll
-        for (int q = 0; q < P; q++) c.p[q] = SHARED_P ? a.p[q] : a.p[(int64_t)q * N + i];
+        for (int q = 0; q < P; q++) c.p[q] = SHARED_P ? a.p[q] : a.p[(int64_t)q * a.N + i];
         return c;
-    };
-    auto sink = [&](int64_t i, const double* res) {
-        if (SHARED_P) {
-#pragma unroll
-            for (int q = 0; q < P; q++) acc[q] += res[q];
-        } else if (lane == 0) {
-#pragma unroll
-            for (int q = 0; q < P; q++) a.dp_members[(int64_t)q * N + i] = res[q];
-        }
-    };
-    quad_member_loop<P>(N, a.K, a.saveat, a.t0, a.t1, a.quad_abstol, a.quad_reltol, a.qseg, a.qkey, a.maxseg, s_quad_l1, make, sink);
-    if (SHARED_P) {
-        if (lane != 0) {
-#pragma unroll
-            for (int q = 0; q < P; q++) acc[q] = 0.0;
-        }
-        reduce_dp<P>(acc, a.partials, a.dp, a.ticket);
-    }
+    });
 }
 
 }  // namespace b200adj

@@ -571,7 +571,7 @@ def test_device_matches_the_reference_under_the_controller(family, sensealg):
 def test_mu_row_time_derivative_cancels_from_interpolating_steps(family):
     """InterpolatingAdjoint's mu rows have W = [.., I]: hd dT_mu enters k1_mu and k3_mu only, and cancels from both the
     solution (k2_mu = f1_mu - hd F'x_lam, free of k1_mu) and the error estimate (k1_mu - 2 k2_mu + k3_mu: +hd dT_mu from k1,
-    -2 hd dT_mu + hd dT_mu from k3).  So ros23_aug_reverse_kernel's dT[D + q] has no effect beyond rounding, and no test of
+    -2 hd dT_mu + hd dT_mu from k3).  So ros23_reverse_kernel's dT[D + q] has no effect beyond rounding, and no test of
     its outputs can see it; the 40-digit reference shows the cancellation, under the controller, to fp64 rounding."""
     a = reference(family, "interpolating", False, False, N_MEMBERS, CTRL_TOL)
     with_zero = reference(family, "interpolating", False, False, N_MEMBERS, CTRL_TOL, drop_mu_dt=True)
