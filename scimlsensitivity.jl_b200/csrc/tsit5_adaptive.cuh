@@ -891,6 +891,9 @@ __global__ void __launch_bounds__(256) t5a_reverse_kernel(const __grid_constant_
         jump_if_at(t);
         event_if_at(t);
     }
+    // the record of the interval below the last lookup may still be on its way (Backsolve's last checkpoint above t0, a
+    // member that stops early): no bulk copy may outlive the CTA whose shared memory it writes
+    if (sol.aiv >= 0) sol.arrived();
     const double qnan = __longlong_as_double(0x7ff8000000000000LL);
     if (active) {
 #pragma unroll

@@ -31,7 +31,7 @@ import numpy as np
 import pytest
 
 from scimlsensitivity_jl_b200 import _lib
-from ros23_restatement import f_ball, f_lorenz, f_lv, f_relax, f_robertson
+from ros23_restatement import dense_interval, f_ball, f_lorenz, f_lv, f_relax, f_robertson, fma
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CSRC = os.path.join(ROOT, "scimlsensitivity.jl_b200", "csrc")
@@ -380,21 +380,6 @@ def test_lu_robertson_w_against_40_digits(probe, adjoint):
 
 # ------------------------------------------------------------------------------------------------------------------------
 # FwdDense<D>::eval
-
-
-def fma(a, b, c):
-    """a * b + c rounded once"""
-    return float(Fraction(a) * Fraction(b) + Fraction(c))
-
-
-def dense_interval(knots, n, t, right):
-    """the interval the cursor search stops on, from a scan of all knots: right = largest idx with T(idx) <= t, left =
-    (smallest idx >= 1 with T(idx) >= t) - 1, clamped to [0, n - 1]"""
-    if right:
-        iv = max([k for k in range(n) if knots[k] <= t], default=0)
-    else:
-        iv = max([k for k in range(n) if k == 0 or knots[k] < t], default=0)
-    return min(max(iv, 0), n - 1)
 
 
 def dense_eval(knots, u, k1, k2, iv, t):

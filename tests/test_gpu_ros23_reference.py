@@ -38,26 +38,19 @@ step is not compared: with 1e30 tolerances its last forward step spans 0.44 of [
 loses 13 digits (the restatement itself moves in the 7th digit between 20 and 40 digits).  The 40-digit reference takes
 ~55 s of host time, GaussKronrod's bisection and the Robertson runs under the controller most of it."""
 import functools
-import os
 
 import numpy as np
 import pytest
 
 import mpmath as mp
 
-from ros23_restatement import f_lorenz, f_lv, f_robertson
+from ros23_restatement import EPS100, f_lorenz, f_lv, f_robertson, problem, register_lv_clone, tstop_snap, vjp_p, vjp_u
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 ROS_D = 0.29289321881345247559915563789515
-EPS100 = 100 * 2.220446049250313e-16
 DPS = 40
 HUGE = 1e30                 # tolerances at which every step is accepted
 COST_A, COST_B = 1.0, -0.5
 FAM = {"lv": (f_lv, 2, 4), "lv_clone": (f_lv, 2, 4), "lorenz": (f_lorenz, 3, 3), "robertson": (f_robertson, 3, 3)}
-
-
-def tstop_snap(tn, ts):
-    return ts if abs(tn - ts) <= EPS100 * max(abs(tn), abs(ts)) else tn
 
 
 def step_factor(eest):
@@ -76,23 +69,6 @@ def _eest(h, k1, k2, k3, x, xn, tol):
         sc = tol + tol * max(abs(x[c]), abs(xn[c]))
         e2 += (e / sc) ** 2
     return mp.sqrt(e2 / len(x))
-
-
-def _problem(family, N, shared_p):
-    """-> (t0, T, saveat, u0[D][N], p[P] or [P][N])"""
-    rng = np.random.default_rng({"lv": 1, "lv_clone": 1, "lorenz": 2, "robertson": 3}[family])
-    if family in ("lv", "lv_clone"):
-        T, u0, p = 2.0, np.exp(0.1 * rng.standard_normal((2, N))), np.array([1.5, 1.0, 3.0, 1.0])
-        saveat = np.linspace(0.25, T, 8)
-    elif family == "lorenz":
-        T, u0, p = 0.5, np.array([1.0, 0.0, 0.0])[:, None] + 0.1 * rng.standard_normal((3, N)), np.array([10.0, 28.0, 8.0 / 3.0])
-        saveat = np.linspace(0.05, T, 10)
-    else:
-        T, u0, p = 10.0, np.repeat(np.array([[1.0], [0.0], [0.0]]), N, 1), np.array([0.04, 3e7, 1e4])
-        saveat = np.logspace(-2, 1, 6)
-    if not shared_p:
-        p = p[:, None] * np.exp(0.05 * rng.standard_normal((len(p), N)))
-    return 0.0, T, saveat, u0, p
 
 
 # ------------------------------------------------------------------------------------------------------------------------
@@ -134,27 +110,6 @@ def _jac_cd(rhs, z):
         for r in range(L):
             A[r, c] = (fp[r] - fm[r]) / (2 * dl)
     return A
-
-
-def _vjp_p(f, y, p, l):
-    """(df/dp)' l by complex steps of l' f(y, p)"""
-    dl = mp.mpf("1e-30")
-    out = []
-    for q in range(len(p)):
-        pc = [mp.mpc(v) for v in p]
-        pc[q] += mp.mpc(0, dl)
-        out.append(mp.im(sum(l[r] * v for r, v in enumerate(f(y, pc)))) / dl)
-    return out
-
-
-def _vjp_u(f, y, p, l):
-    dl = mp.mpf("1e-30")
-    out = []
-    for c in range(len(y)):
-        yc = [mp.mpc(v) for v in y]
-        yc[c] += mp.mpc(0, dl)
-        out.append(mp.im(sum(l[r] * v for r, v in enumerate(f(yc, p)))) / dl)
-    return out
 
 
 # ------------------------------------------------------------------------------------------------------------------------
@@ -242,9 +197,9 @@ def reverse(sensealg, f, fwd, p, saveat, t0, T, every, tol, drop_mu_dt=False):
 
     def rhs(tt, x, iv=None):
         y = x[YO:YO + D] if sensealg == "backsolve" else fwd.eval(tt, True, iv)
-        out = [-v for v in _vjp_u(f, y, p, x[:D])]
+        out = [-v for v in vjp_u(f, y, p, x[:D])]
         if aug:
-            out += [-v for v in _vjp_p(f, y, p, x[:D])]
+            out += [-v for v in vjp_p(f, y, p, x[:D])]
         if sensealg == "backsolve":
             out += f(y, p)
         return out
@@ -330,7 +285,7 @@ def reverse(sensealg, f, fwd, p, saveat, t0, T, every, tol, drop_mu_dt=False):
             return [z[j] + hs * (c1 * k1[j] + c2 * k2[j]) for j in range(D)]
 
         def node(tj):
-            return [-v for v in _vjp_p(f, fwd.eval(tj, False), p, lam(tj))]
+            return [-v for v in vjp_p(f, fwd.eval(tj, False), p, lam(tj))]
 
         if sensealg == "gauss":
             tj = 0.5 * (tn + t)
@@ -411,7 +366,7 @@ def _quad_exact(f, fwd, p, recs, t0, T, D, P):
             c1 = th * (1 - th) / (1 - 2 * mp.mpf(ROS_D))
             c2 = th * (th - 2 * mp.mpf(ROS_D)) / (1 - 2 * mp.mpf(ROS_D))
             lam = [z[j] + hs * (c1 * k1[j] + c2 * k2[j]) for j in range(D)]
-            g = _vjp_p(f, fwd.eval(tj, True, iv), p, lam)
+            g = vjp_p(f, fwd.eval(tj, True, iv), p, lam)
             total = [total[q] + (B - A) / 2 * wi * g[q] for q in range(P)]
     return total
 
@@ -421,7 +376,7 @@ def reference(family, sensealg, shared_p, every, N, tol=HUGE, drop_mu_dt=False):
     """-> dict(du0[D][N], dp[P] or [P][N], fsteps[N], rsteps[N] or None, cond = max cond(W) seen, margin = closest |EEst - 1|
     of any accept/reject decision, rejects = rejected steps, forward and reverse)"""
     f, D, P = FAM[family]
-    t0, T, saveat, u0, p = _problem(family, N, shared_p)
+    t0, T, saveat, u0, p = problem(family, N, shared_p)
     du0, dp, fs, rs, cond = np.zeros((D, N)), np.zeros((P, N)), np.zeros(N, np.int32), np.zeros(N, np.int32), 0.0
     margin, rejects = mp.inf, 0
     with mp.workdps(DPS):
@@ -494,14 +449,7 @@ def test_oracle_matches_the_controller_free_reference(family, sensealg, every):
 
 @pytest.fixture(scope="module")
 def lv_clone_registered():
-    import scimlsensitivity_jl_b200 as b
-    so = os.path.join(ROOT, "examples", "libb200fam_lv_clone.so")
-    if os.path.exists(so):
-        try:
-            return b.register_family(so)
-        except b.B200AdjError:
-            os.remove(so)
-    return b.register_family(b.build_family_plugin(os.path.join(ROOT, "examples", "lv_clone_family.cuh"), "LvClone", "lv_clone", out=so, has_jac=True))
+    return register_lv_clone()
 
 
 @pytest.mark.gpu
