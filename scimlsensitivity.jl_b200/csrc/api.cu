@@ -177,6 +177,17 @@ void build_tsit5_tables(double h, Tsit5Tables* t) {
     for (int j = 0; j < 7; j++) t->hR4[j] = h * R[j][3];
 }
 
+// Weights of tsit5_hermite_c4_du (ode_tsit5.cuh): hR4 with k6 eliminated through du = h sum_{j<6} b_j k_j, in long double.
+void build_c4_du_weights(double h, double* w) {
+    typedef long double LD;
+    double R[7][4];
+    tsit5_weights(0.0, nullptr, R);
+    const LD b6 = TSIT5_A[6][5], r6 = R[5][3];
+    for (int j = 0; j < 5; j++) w[j] = (double)((LD)h * ((LD)R[j][3] - r6 * (LD)TSIT5_A[6][j] / b6));
+    w[5] = (double)(r6 / b6);
+    w[6] = h * R[6][3];
+}
+
 const FamilyVTable* family_lookup(int id) {
     if (id >= 0 && id < BUILTIN_FAMILIES) { const FamilyVTable* vt = &builtin_families()[id]; return vt->abi ? vt : nullptr; }
     auto& r = family_registry();
@@ -922,6 +933,9 @@ int32_t b200adj_reverse(void* handle, const void* dLdu, void* du0, void* dp) {
         a.N = c.N; a.Npad = h->Npad; a.S = h->S; a.trace = h->d_trace;
         for (int j = 0; j < 4; j++) { a.cost_a[j] = (float)h->cost_av[j]; a.cost_b[j] = (float)h->cost_bv[j]; }
         cast_tables(h->tb, &a.tb);
+        double w[7];
+        build_c4_du_weights(c.dt, w);
+        for (int j = 0; j < 7; j++) a.hC4u[j] = (float)w[j];
         a.flags = kernel_flags(h);
         rc = launch(vt->rev_f32, h, a);
     } else if (h->path == Path::FIXED) {
@@ -929,6 +943,7 @@ int32_t b200adj_reverse(void* handle, const void* dLdu, void* du0, void* dp) {
         memset(&a, 0, sizeof(a));
         a.event_of_step = h->d_event_of_step; a.ev_s = h->d_ev_s; a.ev_c = h->d_ev_c; a.ev_ps = h->d_ev_ps; a.ev_pc = h->d_ev_pc; a.nev = h->nev;
         tsit5_weights(0.0, nullptr, a.Rpoly); a.hstep = c.dt;
+        build_c4_du_weights(c.dt, a.hC4u);
         if (c.shared_p && comm_fused_ready(h) && !(c.flags & B200ADJ_FLAG_NCCL_ALLREDUCE) && c.sensealg != B200ADJ_SA_QUADRATURE && !h->has_dgdp && !(h->has_cdgdp && h->cont_on)) {
             // the all-reduce of dp is fused into this kernel's last block (peer-memory mailboxes): no collective launch
             a.p2p = h->p2p; a.p2p.epoch = ++h->p2p_epoch; fused_allreduce = true;

@@ -126,6 +126,7 @@ inline size_t esz(const b200adj_cfg& c) { return c.dtype == B200ADJ_F64 ? sizeof
 
 void tsit5_weights(double th, double* w, double (*Rout)[4] = nullptr);
 void build_tsit5_tables(double h, Tsit5Tables* t);
+void build_c4_du_weights(double h, double* w);     // OdeRevArgsT::hC4u
 template <class T, class S> inline void cast_tables(const S& src, T* dst) {
     for (int i = 0; i < 7; i++) for (int j = 0; j < 6; j++) dst->hA[i][j] = (float)src.hA[i][j];
     for (int i = 0; i < 4; i++) for (int j = 0; j < 7; j++) dst->hBst[i][j] = (float)src.hBst[i][j];

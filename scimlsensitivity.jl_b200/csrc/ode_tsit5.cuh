@@ -102,6 +102,7 @@ template <class R> struct OdeRevArgsT {
     const int32_t* event_of_step; const double* ev_s; const double* ev_c; const double* ev_ps; const double* ev_pc; int32_t nev;   // EV kernels
     R Rpoly[7][4];               // SA_GK: dense-output polynomials b_j(theta) = sum_m Rpoly[j][m] theta^(m+1)
     R hstep;                     // SA_GK: the step size
+    R hC4u[7];                   // tsit5_hermite_c4_du: c4 weights of k1..k5, of du (slot 5, in place of k6) and of k7
     P2PComm p2p;                 // fused cross-GPU all-reduce of dp (nranks <= 1: off)
     Tsit5TablesT<R> tb;
 };
@@ -174,6 +175,22 @@ template <int D, class R> __device__ __forceinline__ void tsit5_hermite_c4(const
 #pragma unroll
         for (int j = 1; j < 7; j++) acc = fma(tb.hR4[j], k[j][i], acc);
         c4[i] = acc;
+    }
+}
+// The same c4 without k6.  u_{n+1} = u_n + sum_{j<6} hA[6][j] k_j (b7 = 0), so k6 = (du - sum_{j<5} hA[6][j] k_j) / hA[6][5]
+// and c4 = sum_{j<5} w_j k_j + w_5 du + hR4[6] k7 with w_j = hR4[j] - hR4[5] b_j / b6 and w_5 = R4[5] / b6 (build_c4_du_weights).
+// A reverse step that has u_{n+1} from the forward pass then rebuilds stages 2..5 only: one RHS call and 5 D stage FMAs
+// fewer.  du carries the rounding of the forward step's sum (about one ulp of u), which |w_5| = 15 and the Hermite
+// weight theta^2 (1-theta)^2 <= 1/16 turn into about one ulp of y.
+template <int D, class R>
+__device__ __forceinline__ void tsit5_hermite_c4_du(const R* w, const R (*k)[D], const R* du, R* c4) {
+#pragma unroll
+    for (int i = 0; i < D; i++) {
+        R acc = w[0] * k[0][i];
+#pragma unroll
+        for (int j = 1; j < 5; j++) acc = fma(w[j], k[j][i], acc);
+        acc = fma(w[5], du[i], acc);
+        c4[i] = fma(w[6], k[6][i], acc);
     }
 }
 template <int D, class R>
@@ -660,13 +677,16 @@ __global__ void __maxnreg__(B200_REV_MAXREG) tsit5_reverse_kernel(const __grid_c
             if (grp < 0) continue;             // resting warp of the rotating row: barriers only
 
             // ---- forward stage recompute on [t_n, t_{n+1}]: the dense-output data of this step ----
+            // k6 only where something needs more than c4: GaussKronrod's general-theta dense output and the event kernels'
+            // left limit (stage 6 re-derived); elsewhere c4 comes from du in its place (tsit5_hermite_c4_du)
+            constexpr bool K6 = EV || SA == SA_GK;
             R tmp[D];
             Fam::f(ulo, p, kf[0]);
             tsit5_stage<D, 1>(tb, ulo, kf, tmp); Fam::f(tmp, p, kf[1]);
             tsit5_stage<D, 2>(tb, ulo, kf, tmp); Fam::f(tmp, p, kf[2]);
             tsit5_stage<D, 3>(tb, ulo, kf, tmp); Fam::f(tmp, p, kf[3]);
             tsit5_stage<D, 4>(tb, ulo, kf, tmp); Fam::f(tmp, p, kf[4]);
-            tsit5_stage<D, 5>(tb, ulo, kf, tmp); Fam::f(tmp, p, kf[5]);
+            if (K6) { tsit5_stage<D, 5>(tb, ulo, kf, tmp); Fam::f(tmp, p, kf[5]); }
 
             if (EV && need_left) {
                 // the step above ended with an event at t_{n+1}: the first adjoint stage sees the LEFT limit there -- the end
@@ -680,9 +700,10 @@ __global__ void __maxnreg__(B200_REV_MAXREG) tsit5_reverse_kernel(const __grid_c
             // Hermite data of the forward dense output: uhi / kf[6] are this step's end point (the checkpoint u_{n+1} and its
             // FSAL derivative, or the re-derived left limit at an event); kf[1..5] are dead from here on (except for GK)
             R du[D], c4[D];
-            tsit5_hermite_c4<D>(tb, kf, c4);
 #pragma unroll
             for (int j = 0; j < D; j++) du[j] = uhi[j] - ulo[j];
+            if (K6) tsit5_hermite_c4<D>(tb, kf, c4);
+            else tsit5_hermite_c4_du<D>(a.hC4u, kf, du, c4);
 #ifdef REV_MIDSYNC
             __syncthreads();
 #endif
