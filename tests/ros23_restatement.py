@@ -2,7 +2,9 @@
 mpmath, bicomplex): the only model input of the Rosenbrock23 and adaptive Tsit5 probes and of the 40-digit reference, which
 derive every derivative from these by differentiation (tests/test_gpu_ros23_probe.py, tests/test_gpu_ros23_reference.py,
 tests/test_gpu_t5a_probe.py).  Also the stepper-independent pieces those tests share: the dense-lookup restatements,
-complex-step VJPs in 40 digits, `tstop_snap`, the test problems and the LvClone plug-in."""
+complex-step VJPs in 40 digits, `tstop_snap`, the test problems, the LvClone plug-in and the Tsit5 tableau as published
+(tests/test_tsit5_hermite_tables.py, tests/test_gpu_t5a_probe.py, tests/test_gpu_fixed_probe.py,
+tests/test_gpu_fixed_reference.py)."""
 import os
 from fractions import Fraction
 
@@ -12,6 +14,52 @@ import mpmath as mp
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 EPS100 = 100 * 2.220446049250313e-16
+
+# Tsit5 (Tsitouras 2011), as published: A (row 6 = b, b_7 = 0), c, and the embedded error weights btilde = b - bhat
+A_TXT = [[], ["0.161"], ["-0.008480655492356989", "0.335480655492357"],
+         ["2.897153057105493", "-6.359448489975075", "4.3622954328695815"],
+         ["5.325864828439257", "-11.748883564062828", "7.4955393428898365", "-0.09249506636175525"],
+         ["5.86145544294642", "-12.92096931784711", "8.159367898576159", "-0.071584973281401", "-0.028269050394068383"],
+         ["0.09646076681806523", "0.01", "0.4798896504144996", "1.379008574103742", "-3.290069515436081", "2.324710524099774"]]
+C_TXT = ["0.0", "0.161", "0.327", "0.9", "0.9800255409045097", "1.0", "1.0"]
+BT_TXT = ["-0.00178001105222577714", "-0.0008164344596567469", "0.007880878010261995", "-0.1447110071732629",
+          "0.5823571654525552", "-0.45808210592918697", "0.015151515151515152"]
+
+
+def b_exact(j, th):
+    """Tsit5 dense-output weight b_j(theta), the published factored form, exact at the given theta (float or Fraction)"""
+    t = Fraction(th)
+    F = Fraction
+    if j == 0:
+        return F("-1.0530884977290216") * t * (t - F("1.3299890189751412")) * (t * t - F("1.4364028541716351") * t + F("0.7139816917074209"))
+    if j in (1, 2):
+        c, s, w = {1: ("0.1017", "2.1966568338249754", "1.2949852507374631"),
+                   2: ("2.490627285651252793", "2.38535645472061657", "1.57803468208092486")}[j]
+        return F(c) * t * t * (t * t - F(s) * t + F(w))
+    c, r1, r2 = {3: ("-16.54810288924490272", "1.21712927295533244", "0.61620406037800089"),
+                 4: ("47.37952196281928122", "1.203071208372362603", "0.658047292653547382"),
+                 5: ("-34.87065786149660974", "1.2", "0.666666666666666667"),
+                 6: ("2.5", "1.0", "0.6")}[j]
+    return F(c) * (t - F(r1)) * (t - F(r2)) * t * t
+
+
+def _r_exact():
+    """R[j][m]: b_j(theta) = sum_m R[j][m] theta^(m+1), from the factored b_exact at theta = 1..4 (exact rationals)"""
+    R = []
+    for j in range(7):
+        M = [[Fraction(th) ** (m + 1) for m in range(4)] + [b_exact(j, th)] for th in (1, 2, 3, 4)]
+        for c in range(4):
+            for r in range(c + 1, 4):
+                f = M[r][c] / M[c][c]
+                M[r] = [M[r][k] - f * M[c][k] for k in range(5)]
+        x = [Fraction(0)] * 4
+        for c in range(3, -1, -1):
+            x[c] = (M[c][4] - sum(M[c][k] * x[k] for k in range(c + 1, 4))) / M[c][c]
+        R.append(x)
+    return R
+
+
+R_EXACT = _r_exact()
 
 
 def f_lv(u, p):

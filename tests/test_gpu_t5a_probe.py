@@ -46,8 +46,8 @@ import pytest
 import mpmath as mp
 
 from scimlsensitivity_jl_b200 import _lib
-from ros23_restatement import EPS100, dense_interval, f_lorenz, f_lv, f_robertson, fma, problem, register_lv_clone, tstop_snap, vjp_u
-from test_tsit5_hermite_tables import b_exact
+from ros23_restatement import (A_TXT, BT_TXT, C_TXT, EPS100, R_EXACT, b_exact, dense_interval, f_lorenz, f_lv, f_robertson, fma, problem,
+                               register_lv_clone, tstop_snap, vjp_u)
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CSRC = os.path.join(ROOT, "scimlsensitivity.jl_b200", "csrc")
@@ -55,35 +55,7 @@ PROBE = os.path.join(ROOT, "tests", "csrc", "t5a_probe.cu")
 EPS = 2.220446049250313e-16
 DPS = 40
 
-# Tsit5 (Tsitouras 2011), as published: A (row 6 = b, b_7 = 0), c, and the embedded error weights btilde = b - bhat
-A_TXT = [[], ["0.161"], ["-0.008480655492356989", "0.335480655492357"],
-         ["2.897153057105493", "-6.359448489975075", "4.3622954328695815"],
-         ["5.325864828439257", "-11.748883564062828", "7.4955393428898365", "-0.09249506636175525"],
-         ["5.86145544294642", "-12.92096931784711", "8.159367898576159", "-0.071584973281401", "-0.028269050394068383"],
-         ["0.09646076681806523", "0.01", "0.4798896504144996", "1.379008574103742", "-3.290069515436081", "2.324710524099774"]]
-C_TXT = ["0.0", "0.161", "0.327", "0.9", "0.9800255409045097", "1.0", "1.0"]
-BT_TXT = ["-0.00178001105222577714", "-0.0008164344596567469", "0.007880878010261995", "-0.1447110071732629",
-          "0.5823571654525552", "-0.45808210592918697", "0.015151515151515152"]
 C64 = [float(c) for c in C_TXT]
-
-
-def _r_exact():
-    """R[j][m]: b_j(theta) = sum_m R[j][m] theta^(m+1), from the factored b_exact at theta = 1..4 (exact rationals)"""
-    R = []
-    for j in range(7):
-        M = [[Fraction(th) ** (m + 1) for m in range(4)] + [b_exact(j, float(th))] for th in (1, 2, 3, 4)]
-        for c in range(4):
-            for r in range(c + 1, 4):
-                f = M[r][c] / M[c][c]
-                M[r] = [M[r][k] - f * M[c][k] for k in range(5)]
-        x = [Fraction(0)] * 4
-        for c in range(3, -1, -1):
-            x[c] = (M[c][4] - sum(M[c][k] * x[k] for k in range(c + 1, 4))) / M[c][c]
-        R.append(x)
-    return R
-
-
-R_EXACT = _r_exact()
 FAMS = {"lv": (f_lv, 2, 4), "lv_clone": (f_lv, 2, 4), "lorenz": (f_lorenz, 3, 3), "robertson": (f_robertson, 3, 3)}
 
 
