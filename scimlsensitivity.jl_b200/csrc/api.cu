@@ -271,16 +271,15 @@ void free_all(Handle* h) {
     if (h->own_stream) cudaStreamDestroy(h->own_stream);
 }
 
-// the continuous callback's per-member event lists for max_events events: times cc_t, counts cc_n and, for the family's own
-// conditions (words = true), the event words cc_ev
-int32_t cc_lists(Handle* h, int32_t max_events, bool words) {
+// the continuous callback's per-member event lists for max_events events: times cc_t, counts cc_n and event words cc_ev
+int32_t cc_lists(Handle* h, int32_t max_events) {
     const size_t N = (size_t)h->cfg.N, E = (size_t)max_events;
-    if (E != (size_t)h->cc_maxev || !h->d_cc_t) {
+    if (E != (size_t)h->cc_maxev || !h->d_cc_ev) {      // (cc_ev is allocated last: set only when all three are)
         cudaFree(h->d_cc_t); cudaFree(h->d_cc_n); cudaFree(h->d_cc_ev); h->d_cc_t = nullptr; h->d_cc_n = nullptr; h->d_cc_ev = nullptr; h->cc_on = false;
         CUDA_TRY(h, cudaMalloc(&h->d_cc_t, E * N * sizeof(double)));
         CUDA_TRY(h, cudaMalloc(&h->d_cc_n, N * sizeof(int32_t)));
+        CUDA_TRY(h, cudaMalloc(&h->d_cc_ev, E * N * sizeof(int32_t)));
     }
-    if (words && !h->d_cc_ev) CUDA_TRY(h, cudaMalloc(&h->d_cc_ev, E * N * sizeof(int32_t)));
     CUDA_TRY(h, cudaMemsetAsync(h->d_cc_n, 0, N * sizeof(int32_t), h->stream));
     return B200ADJ_OK;
 }
@@ -692,7 +691,7 @@ int32_t b200adj_set_continuous_callback(void* handle, int32_t enabled, int32_t i
     if (c.d > 4) { h->err = "continuous callback: d <= 4"; return B200ADJ_ERR_UNSUPPORTED; }
     if (idx < 0 || idx >= c.d || direction < -1 || direction > 1 || pcomp >= c.d || (pcomp >= 0 && (pparam < 0 || pparam >= c.P)) || max_events < 1 ||
         !std::isfinite(level) || !std::isfinite(psign)) { h->err = "continuous callback: bad idx / direction / pcomp / pparam / max_events"; return B200ADJ_ERR_INVALID; }
-    if (int32_t rc = cc_lists(h, max_events, false)) return rc;
+    if (int32_t rc = cc_lists(h, max_events)) return rc;
     h->fe_nc = 0;                     // the named condition and affect
     h->cc_on = true; h->cc_idx = idx; h->cc_dir = direction; h->cc_pcomp = pcomp < 0 ? -1 : pcomp; h->cc_pparam = pcomp < 0 ? 0 : pparam;
     h->cc_maxev = max_events; h->cc_level = level; h->cc_psign = psign;
@@ -757,7 +756,7 @@ int32_t b200adj_set_family_events(void* handle, int32_t enabled, int32_t nc, con
     if (nc != vt->nc || !direction || max_events < 1) { h->err = "family events: nc differs from the family's, null direction or max_events < 1"; return B200ADJ_ERR_INVALID; }
     for (int k = 0; k < nc; k++)
         if (direction[k] < -1 || direction[k] > 1) { h->err = "family events: a direction is outside {-1, 0, 1}"; return B200ADJ_ERR_INVALID; }
-    if (int32_t rc = cc_lists(h, max_events, true)) return rc;
+    if (int32_t rc = cc_lists(h, max_events)) return rc;
     h->cc_on = true; h->cc_maxev = max_events; h->fe_nc = nc;
     for (int k = 0; k < 8; k++) h->fe_dir[k] = k < nc ? direction[k] : 0;
     h->have_forward = false;

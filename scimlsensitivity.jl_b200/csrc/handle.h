@@ -78,14 +78,14 @@ struct Handle {
     int32_t* d_ev_ac = nullptr; int32_t* d_ev_ak = nullptr; double* d_ev_af = nullptr;      // b200adj_set_event_param_shift
     int32_t* d_event_of_step = nullptr;     // fixed-step Tsit5: event index at grid point n, or -1
     int nev = 0; double *d_ev_t = nullptr, *d_ev_s = nullptr, *d_ev_c = nullptr, *d_ev_ps = nullptr, *d_ev_pc = nullptr;      // preset-time events
-    // state-dependent event (b200adj_set_continuous_callback): per-member event lists cc_t[cc_maxev][N], cc_n[N]
+    // state-dependent event (b200adj_set_continuous_callback): per-member event lists cc_t[cc_maxev][N], cc_n[N] and the
+    // event words cc_ev[cc_maxev][N] of the events found
     bool cc_on = false; int cc_idx = 0, cc_dir = 0, cc_pcomp = -1, cc_pparam = 0, cc_maxev = 0;
     double cc_level = 0, cc_psign = 1, cc_scale[4] = {1, 1, 1, 1}, cc_shift[4] = {0, 0, 0, 0};
     int cc_lparam = -1, cc_acomp = -1, cc_aparam = 0, cc_qcomp = -1; double cc_lcoef = 0, cc_acoef = 0, cc_qcoef = 1;      // b200adj_set_continuous_callback_params
-    double* d_cc_t = nullptr; int32_t* d_cc_n = nullptr;
-    // the callback's family mode (b200adj_set_family_events): fe_nc > 0 conditions of the family, their directions, and the
-    // event words cc_ev[cc_maxev][N] of the events found
-    int fe_nc = 0; int32_t fe_dir[8] = {0}; int32_t* d_cc_ev = nullptr;
+    double* d_cc_t = nullptr; int32_t* d_cc_n = nullptr; int32_t* d_cc_ev = nullptr;
+    // the callback's family mode (b200adj_set_family_events): fe_nc > 0 conditions of the family and their directions
+    int fe_nc = 0; int32_t fe_dir[8] = {0};
     int rev_block = 0; const void* rev_block_kernel = nullptr;      // adaptive Tsit5 reverse kernel: block size chosen per instantiation (disp_t5a.inc)
     bool have_forward = false;
     bool noise_valid = false;

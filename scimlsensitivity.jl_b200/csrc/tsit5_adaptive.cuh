@@ -10,6 +10,7 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <type_traits>
 #include "families.cuh"
 #include "ode_tsit5.cuh"
 #include "ros23.cuh"
@@ -41,7 +42,8 @@ struct T5aArgs {
     // state-dependent event (ContinuousCallback, src/callback_tracking.jl:232-480; docs/src/examples/hybrid_jump/bouncing_ball.md):
     // condition u[cc_idx] - cc_level crossing zero in direction cc_dir (-1 down, +1 up, 0 both); affect u <- cc_scale .* u +
     // cc_shift, then u[cc_pcomp] <- cc_psign * p[cc_pparam] * u[cc_pcomp] (cc_pcomp < 0: none).  The forward kernel (CC = true)
-    // FINDS each member's event times: cc_t[cc_maxev][N], cc_n[N]; the reverse kernel reads them as member-local tstops.
+    // FINDS each member's event times: cc_t[cc_maxev][N], cc_n[N], with each its event word cc_ev[cc_maxev][N] (bit 2c =
+    // condition c fired, bit 2c + 1 = it crossed upwards); the reverse kernel reads them as member-local tstops.
     int32_t cc_on, cc_idx, cc_dir, cc_pcomp, cc_pparam, cc_maxev;
     double cc_level, cc_psign, cc_scale[4], cc_shift[4];
     double* cc_t; int32_t* cc_n;
@@ -55,8 +57,7 @@ struct T5aArgs {
     double R[7][4];         // dense-output polynomials: b_j(theta) = sum_m R[j][m] theta^(m+1)
     // family events (VectorContinuousCallback, b200adj_set_family_events): the continuous callback's conditions and affect are
     // the ones compiled into the family struct (Fam::NC, condition, condition_grad, affect, affect_vjp; family_plugin.inc).
-    // fe_nc > 0 selects them; fe_dir[c] is the direction of condition c (-1 down, +1 up, 0 both).  The forward kernel stores
-    // with each event time of cc_t its event word cc_ev[cc_maxev][N]: bit 2c = condition c fired, bit 2c + 1 = it crossed upwards.
+    // fe_nc > 0 selects them; fe_dir[c] is the direction of condition c (-1 down, +1 up, 0 both).
     int32_t fe_nc, fe_dir[8];
     int32_t* cc_ev;
 };
@@ -234,16 +235,70 @@ __device__ __forceinline__ double t5_pick(const double* v, int idx) {
     return r;
 }
 
-// Condition policy of the state-dependent event: NC conditions g_c(y, p, t), each with its direction -- here the conditions
-// compiled into the family (b200adj_set_family_events).  (The named condition u[cc_idx] - level keeps its own scalar loop in
-// t5a_forward_kernel: routed through t5_find_event it compiles to different SASS, and its kernels are pinned.)
+// Event policy of the continuous callback, the interface of family_plugin.inc: NC conditions g_c(y, p, t), each with its
+// direction dir(c), their gradients, the affect and its VJP.  Both kinds of callback run the same event search
+// (t5_find_event) and the same saltation (t5a_reverse_kernel).
+// The conditions and affect compiled into the family (b200adj_set_family_events).
 template <class Fam>
-struct T5FamilyCond {
+struct T5FamilyEvent {
     static constexpr int NC = Fam::NC;
     const T5aArgs& a;
-    __device__ __forceinline__ void operator()(const double* y, const double* p, double t, double* g) const { Fam::condition(y, p, t, g); }
     __device__ __forceinline__ int dir(int c) const { return a.fe_dir[c]; }
+    __device__ __forceinline__ void condition(const double* y, const double* p, double t, double* g) const { Fam::condition(y, p, t, g); }
+    __device__ __forceinline__ double condition_grad(int c, const double* u, const double* p, double t, double* gu, double* gp) const {
+        return Fam::condition_grad(c, u, p, t, gu, gp);
+    }
+    __device__ __forceinline__ void affect(const int* ev, const double* um, const double* p, double* up) const { Fam::affect(ev, um, p, up); }
+    __device__ __forceinline__ void affect_vjp(const int* ev, const double* um, const double* p, const double* l, double* lu, double* lp) const {
+        Fam::affect_vjp(ev, um, p, l, lu, lp);
+    }
 };
+// The named callback (b200adj_set_continuous_callback / _params): the condition u[cc_idx] - (cc_level + cc_lcoef p[cc_lparam])
+// and the affect of t5_cc_affect, with u[cc_qcomp] <- cc_qcoef u[cc_qcomp]^2 in place of that component's affine map
+template <int D, int P>
+struct T5NamedEvent {
+    static constexpr int NC = 1;
+    const T5aArgs& a;
+    __device__ __forceinline__ int dir(int) const { return a.cc_dir; }
+    __device__ __forceinline__ void condition(const double* y, const double* p, double, double* g) const {
+        g[0] = t5_pick<D>(y, a.cc_idx) - t5_cc_level<P>(a, p);
+    }
+    __device__ __forceinline__ double condition_grad(int, const double*, const double*, double, double* gu, double* gp) const {
+#pragma unroll
+        for (int j = 0; j < D; j++) gu[j] = (j == a.cc_idx) ? 1.0 : 0.0;
+#pragma unroll
+        for (int q = 0; q < P; q++) gp[q] = (q == a.cc_lparam) ? -a.cc_lcoef : 0.0;
+        return 0.0;
+    }
+    __device__ __forceinline__ void affect(const int*, const double* um, const double* p, double* up) const {
+        double sc[D], sh[D];
+        t5_cc_affect<D, P>(a, p, sc, sh);
+#pragma unroll
+        for (int j = 0; j < D; j++) up[j] = (j == a.cc_qcomp) ? a.cc_qcoef * um[j] * um[j] : sc[j] * um[j] + sh[j];
+    }
+    // the affect is diagonal in u: lu = sc .* l (2 qcoef u-[qcomp] for the quadratic component); lp from u[pcomp] <- psign p[pparam]
+    // u[pcomp] and u[acomp] += acoef p[aparam]
+    __device__ __forceinline__ void affect_vjp(const int*, const double* um, const double* p, const double* l, double* lu, double* lp) const {
+        double sc[D], sh[D];
+        t5_cc_affect<D, P>(a, p, sc, sh);
+#pragma unroll
+        for (int j = 0; j < D; j++) lu[j] = ((j == a.cc_qcomp) ? 2.0 * a.cc_qcoef * um[j] : sc[j]) * l[j];
+#pragma unroll
+        for (int q = 0; q < P; q++) lp[q] = 0.0;
+        if (a.cc_pcomp >= 0) {
+            const double gpar = a.cc_psign * t5_pick<D>(um, a.cc_pcomp) * t5_pick<D>(l, a.cc_pcomp);
+#pragma unroll
+            for (int q = 0; q < P; q++) if (q == a.cc_pparam) lp[q] += gpar;
+        }
+        if (a.cc_acomp >= 0) {
+            const double gadd = a.cc_acoef * t5_pick<D>(l, a.cc_acomp);
+#pragma unroll
+            for (int q = 0; q < P; q++) if (q == a.cc_aparam) lp[q] += gadd;
+        }
+    }
+};
+template <class Fam, bool FE>
+using T5Event = std::conditional_t<FE, T5FamilyEvent<Fam>, T5NamedEvent<Fam::D, Fam::P>>;
 
 // Event search on one accepted step [t, t + h] (k1..k7 in registers, un = the end point): the conditions are evaluated on the
 // dense output y(theta) at theta = j / 10 (interp_points = 10 of ContinuousCallback: a long step may hold a whole flight);
@@ -253,11 +308,11 @@ struct T5FamilyCond {
 // side from the first sample instead.  Returns the event word (bit 2c fired, bit 2c + 1 upwards; 0 = no event) and theta*;
 // *pending gets the same bits for the conditions that cross in that interval but whose roots have other bits
 // (t5_fire_reached decides them once the step is redone).
-template <int D, class Cond>
-__device__ __forceinline__ uint32_t t5_find_event(const T5aArgs& a, const Cond& cond, const double* u, const double* un,
+template <int D, class Event>
+__device__ __forceinline__ uint32_t t5_find_event(const T5aArgs& a, const Event& event, const double* u, const double* un,
                                                   const double (*k)[D], const double* p, double t, double h, uint32_t skip, double* thstar,
                                                   uint32_t* pending) {
-    constexpr int NC = Cond::NC;
+    constexpr int NC = Event::NC;
     auto conds_at = [&](double th, double* g) {         // the full dense output y(theta), once per sample
         double y[D], w[7];
         t5_weights(a, th, w);
@@ -268,18 +323,18 @@ __device__ __forceinline__ uint32_t t5_find_event(const T5aArgs& a, const Cond& 
             for (int s = 0; s < 7; s++) acc += w[s] * k[s][j];
             y[j] = u[j] + h * acc;
         }
-        cond(y, p, t + th * h, g);
+        event.condition(y, p, t + th * h, g);
     };
     double gprev[NC], gj[NC], thprev = 0.0, lo = 0.0, hi = 1.0;
-    cond(u, p, t, gprev);
+    event.condition(u, p, t, gprev);
     uint32_t cross = 0;
     for (int j = 1; j <= 10 && !cross; j++) {
         const double th = j == 10 ? 1.0 : 0.1 * j;
-        if (j == 10) cond(un, p, t + h, gj); else conds_at(th, gj);
+        if (j == 10) event.condition(un, p, t + h, gj); else conds_at(th, gj);
 #pragma unroll
         for (int c = 0; c < NC; c++) {
             if (j == 1 && ((skip >> c) & 1u)) continue;
-            const int dr = cond.dir(c);
+            const int dr = event.dir(c);
             if ((dr <= 0 && gprev[c] > 0 && gj[c] <= 0) || (dr >= 0 && gprev[c] < 0 && gj[c] >= 0)) cross |= 1u << c;
         }
         if (cross) { lo = thprev; hi = th; }
@@ -325,22 +380,24 @@ __device__ __forceinline__ uint32_t t5_find_event(const T5aArgs& a, const Cond& 
 // The conditions of `pending` whose value at the end point un of the redone step (time tn) has reached their far side or
 // zero fire with the event.  The next step starts from un, and a condition that starts there on its far side or on zero can
 // never satisfy the crossing test: a root a few ulps after theta* would otherwise be lost (its affect silently skipped).
-template <class Fam>
-__device__ __forceinline__ uint32_t t5_fire_reached(const double* un, const double* p, double tn, uint32_t pending) {
+template <class Event>
+__device__ __forceinline__ uint32_t t5_fire_reached(const Event& event, const double* un, const double* p, double tn, uint32_t pending) {
     if (!pending) return 0u;
-    double g[Fam::NC];
-    Fam::condition(un, p, tn, g);
+    double g[Event::NC];
+    event.condition(un, p, tn, g);
     uint32_t word = 0;
 #pragma unroll
-    for (int c = 0; c < Fam::NC; c++)
+    for (int c = 0; c < Event::NC; c++)
         if (fe_fired(pending, c) && (fe_upward(pending, c) ? g[c] >= 0 : g[c] <= 0)) word |= pending & (3u << (2 * c));
     return word;
 }
 
-// CC: state-dependent event; FE (with CC): its conditions and affect are those of the family (T5FamilyCond), else named
+// CC: continuous callback, its conditions and affect those of the policy T5Event<Fam, FE>: the family's (FE) or the named one
 template <class Fam, bool SHARED_P, bool CC = false, bool FE = false>
 __global__ void __launch_bounds__(256) t5a_forward_kernel(const __grid_constant__ T5aArgs a) {
     constexpr int D = Fam::D, P = Fam::P;
+    using Event = T5Event<Fam, FE>;
+    const Event event{a};
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= a.N) return;
     const int64_t N = a.N;
@@ -368,24 +425,8 @@ __global__ void __launch_bounds__(256) t5a_forward_kernel(const __grid_constant_
     }
     int ev = 0;                                   // next event ahead of t (event times are tstops of the forward solve)
     const bool fixed = (a.flags & KF_FIXED_DT) != 0;      // constant step dt0, no error control (fixed-step Tsit5 with off-grid save times)
-    bool after_event = false;                     // CC: the step starts on an event (condition ~0 with a random sign)
     int nfound = 0;
-    const double cc_lev = (CC && !FE) ? t5_cc_level<P>(a, p) : 0.0;
-    uint32_t fe_skip = 0, fe_word = 0;            // FE: conditions that fired at the event the step starts on; the event word
-    // component cc_idx of the step's dense output at theta (k1..k7 in registers)
-    auto cond_at = [&](double th, double hh) {
-        double w[7];
-        t5_weights(a, th, w);
-        double r = 0.0;
-#pragma unroll
-        for (int j = 0; j < D; j++) {
-            double acc = 0.0;
-#pragma unroll
-            for (int s = 0; s < 7; s++) acc += w[s] * k[s][j];
-            if (j == a.cc_idx) r = u[j] + hh * acc;
-        }
-        return r - cc_lev;
-    };
+    uint32_t cc_skip = 0, cc_word = 0;            // CC: conditions that fired at the event the step starts on; the event word
     while (t < a.t1) {
         if (++iters > 10000000L || n >= a.maxs) { stat = 2; break; }
         bool last = false;
@@ -404,13 +445,14 @@ __global__ void __launch_bounds__(256) t5a_forward_kernel(const __grid_constant_
         if (EEst <= 1.0) {
             double tn = last ? tend : t + h;
             bool at_event = !CC && last && ev < a.nev;
-            if constexpr (FE) {
-                // the family's conditions (t5_find_event): right after an event the conditions that fired there take their
-                // side from the first sample; the step is redone up to theta* as below
+            if constexpr (CC) {
+                // the callback's conditions (t5_find_event): right after an event the conditions that fired there take their
+                // side from the first sample; the step is redone up to theta* so that the stored dense data belong to [t, tau]
+                // (k[0] = f(u) is still valid)
                 double thstar = 1.0;
                 uint32_t pend = 0;
-                uint32_t word = t5_find_event<D>(a, T5FamilyCond<Fam>{a}, u, un, k, p, t, h, fe_skip, &thstar, &pend);
-                fe_skip = 0;
+                uint32_t word = t5_find_event<D>(a, event, u, un, k, p, t, h, cc_skip, &thstar, &pend);
+                cc_skip = 0;
                 if (word) {
                     // an event never lands on the time of the one before (a root a few ulps into the step, right after an
                     // event): the reverse pass tells events and their dense intervals apart by their times
@@ -418,43 +460,12 @@ __global__ void __launch_bounds__(256) t5a_forward_kernel(const __grid_constant_
                     if (!(t + hh > t)) hh = fmax(fabs(t), 1e-300) * 2.220446049250313e-16;      // >= one ulp of t
                     t5_step<D>(a, rhs, t, hh, u, k, un);
                     tn = t + hh;
-                    word |= t5_fire_reached<Fam>(un, p, tn, pend);
+                    word |= t5_fire_reached(event, un, p, tn, pend);
                     at_event = true;
                     if (nfound >= a.cc_maxev) { stat = 3; break; }
                     a.cc_t[(int64_t)nfound * N + i] = tn;
                     a.cc_ev[(int64_t)nfound * N + i] = (int32_t)word;
-                    fe_word = word;
-                    nfound++;
-                }
-            } else if (CC) {
-                // sign changes of the condition on the dense output, sampled at theta = j / 10 (interp_points = 10 of
-                // ContinuousCallback: a long step may hold a whole flight); right after an event the first sample decides the side
-                double gprev = t5_pick<D>(u, a.cc_idx) - cc_lev, thprev = 0.0, lo = 0.0, hi = 1.0;
-                bool hit = false;
-                for (int j = 1; j <= 10 && !hit; j++) {
-                    const double th = j == 10 ? 1.0 : 0.1 * j;
-                    const double gj = (j == 10) ? t5_pick<D>(un, a.cc_idx) - cc_lev : cond_at(th, h);
-                    if (after_event && j == 1) { gprev = gj; thprev = th; continue; }
-                    if ((a.cc_dir <= 0 && gprev > 0 && gj <= 0) || (a.cc_dir >= 0 && gprev < 0 && gj >= 0)) { hit = true; lo = thprev; hi = th; }
-                    else { gprev = gj; thprev = th; }
-                }
-                after_event = false;
-                if (hit) {
-                    // bisection of the crossing to the last bit, then the step is REDONE with h' = theta* h so that the stored
-                    // dense data belong to [t, tau] (k[0] = f(u) is still valid)
-                    const bool pos = gprev > 0;
-                    for (int it = 0; it < 200; it++) {
-                        const double mid = 0.5 * (lo + hi);
-                        if (!(mid > lo && mid < hi)) break;
-                        const double gm = cond_at(mid, h);
-                        if ((gm > 0) == pos && gm != 0) lo = mid; else hi = mid;
-                    }
-                    const double hh = hi * h;
-                    t5_step<D>(a, rhs, t, hh, u, k, un);
-                    tn = t + hh;
-                    at_event = true;
-                    if (nfound >= a.cc_maxev) { stat = 3; break; }
-                    a.cc_t[(int64_t)nfound * N + i] = tn;
+                    cc_word = word;
                     nfound++;
                 }
             }
@@ -500,24 +511,18 @@ __global__ void __launch_bounds__(256) t5a_forward_kernel(const __grid_constant_
             }
             if (at_event) {
                 // affect!: the next step starts from the post-event state; k7 = f(u^-) stays with the step just stored
-                if constexpr (FE) {
-                    // affect!(integrator, ev) of the family: ev[c] = +1 / -1 for a condition that crossed upwards / downwards
-                    int evs[Fam::NC];
+                if constexpr (CC) {
+                    // affect!(integrator, ev): ev[c] = +1 / -1 for a condition that crossed upwards / downwards
+                    int evs[Event::NC];
                     double up[D];
 #pragma unroll
-                    for (int c = 0; c < Fam::NC; c++) evs[c] = fe_fired(fe_word, c) ? (fe_upward(fe_word, c) ? 1 : -1) : 0;
-                    Fam::affect(evs, un, p, up);
+                    for (int c = 0; c < Event::NC; c++) evs[c] = fe_fired(cc_word, c) ? (fe_upward(cc_word, c) ? 1 : -1) : 0;
+                    event.affect(evs, un, p, up);
 #pragma unroll
                     for (int j = 0; j < D; j++) un[j] = up[j];
-                    fe_skip = 0;
+                    cc_skip = 0;
 #pragma unroll
-                    for (int c = 0; c < Fam::NC; c++) fe_skip |= fe_fired(fe_word, c) << c;
-                } else if (CC) {
-                    double sc[D], sh[D];
-                    t5_cc_affect<D, P>(a, p, sc, sh);
-#pragma unroll
-                    for (int j = 0; j < D; j++) un[j] = (j == a.cc_qcomp) ? a.cc_qcoef * un[j] * un[j] : sc[j] * un[j] + sh[j];
-                    after_event = true;
+                    for (int c = 0; c < Event::NC; c++) cc_skip |= fe_fired(cc_word, c) << c;
                 } else {
 #pragma unroll
                 for (int j = 0; j < D; j++) un[j] = a.ev_s[ev * D + j] * un[j] + a.ev_c[ev * D + j];
@@ -669,13 +674,14 @@ __global__ void __launch_bounds__(256) t5a_reverse_kernel(const __grid_constant_
     // solution (the reference keeps it as `uleft` of the TrackedAffect).  Runs after the checkpoint reset and the loss jump.
     auto event_if_at = [&](double tt) {
         while (evc >= 0 && fabs(evt(evc) - tt) <= EPS100 * fmax(fabs(tt), 1.0)) {
-            if constexpr (FE) {
-                // state-dependent event of the family's conditions and affect (the implicit event-time correction of
+            if constexpr (CC) {
+                // state-dependent event of the callback's conditions and affect (the implicit event-time correction of
                 // src/callback_tracking.jl:232-480): with u+ = a(u-, p), c = the lowest condition that fired, g_c(u-, p, tau) = 0,
                 //   (mu_u, mu_p) = ((da/du)'lam+, (da/dp)'lam+),  den = dg/du . f(u-) + dg/dt,  w = mu_u . f(u-) - lam+ . f(u+)
                 //   lam- = mu_u - dg/du (w / den),  dG/dp += mu_p - dg/dp (w / den)
-                // For g = u_i - level - lcoef p_k and a diagonal affect this is the named formula of the branch below.
-                constexpr int NC = Fam::NC;
+                using Event = T5Event<Fam, FE>;
+                constexpr int NC = Event::NC;
+                const Event event{a};
                 double um[D], up[D], fm[D], fp[D], mu[D], mp[P], gu[D], gp[P];
                 const double tau = evt(evc);
                 sol.eval(tau, false, um); sol.eval(tau, true, up);
@@ -687,8 +693,8 @@ __global__ void __launch_bounds__(256) t5a_reverse_kernel(const __grid_constant_
                     evs[c] = fe_fired(word, c) ? (fe_upward(word, c) ? 1 : -1) : 0;
                     if (evs[c]) cf = c;
                 }
-                Fam::affect_vjp(evs, um, p, z, mu, mp);
-                const double gt = Fam::condition_grad(cf, um, p, tau, gu, gp);
+                event.affect_vjp(evs, um, p, z, mu, mp);
+                const double gt = event.condition_grad(cf, um, p, tau, gu, gp);
                 double den = gt, w = 0.0;
 #pragma unroll
                 for (int j = 0; j < D; j++) { den += gu[j] * fm[j]; w += mu[j] * fm[j] - z[j] * fp[j]; }
@@ -700,49 +706,6 @@ __global__ void __launch_bounds__(256) t5a_reverse_kernel(const __grid_constant_
                 }
 #pragma unroll
                 for (int j = 0; j < D; j++) z[j] = mu[j] - gu[j] * r;
-                if (SA == SA_BACKSOLVE) {
-#pragma unroll
-                    for (int j = 0; j < D; j++) z[YO + j] = um[j];
-                }
-            } else if constexpr (CC) {
-                // state-dependent event time (the implicit correction of src/callback_tracking.jl:232-480): with u+ = A u- + c,
-                // g(u-) = 0:  lam- = A'lam+ - e_ci [(A f- - f+)'lam+] / f-[ci],   dG/dp += (dA/dp u-)'lam+
-                double um[D], up[D], fm[D], fp[D], sc[D], sh[D];
-                const double tau = evt(evc);
-                sol.eval(tau, false, um); sol.eval(tau, true, up);
-                Fam::f(um, p, fm); Fam::f(up, p, fp);
-                t5_cc_affect<D, P>(a, p, sc, sh);
-                if (a.cc_qcomp >= 0) {       // u_q <- qcoef u_q^2: the Jacobian 2 qcoef u_q- takes the place of the scale
-#pragma unroll
-                    for (int j = 0; j < D; j++) if (j == a.cc_qcomp) sc[j] = 2.0 * a.cc_qcoef * um[j];
-                }
-                double wl = 0.0;
-#pragma unroll
-                for (int j = 0; j < D; j++) wl += (sc[j] * fm[j] - fp[j]) * z[j];
-                if (a.cc_pcomp >= 0) {
-                    const double gpar = a.cc_psign * t5_pick<D>(um, a.cc_pcomp) * t5_pick<D>(z, a.cc_pcomp);
-#pragma unroll
-                    for (int q = 0; q < P; q++) if (q == a.cc_pparam) {
-                        if (SA == SA_INTERP || SA == SA_BACKSOLVE) z[D + (L > D ? q : 0)] += gpar; else acc[q] += gpar;
-                    }
-                }
-                const double corr = wl / t5_pick<D>(fm, a.cc_idx);
-                if (a.cc_acomp >= 0) {       // u+[acomp] += acoef p[aparam]: (da/dp)'lam+
-                    const double gadd = a.cc_acoef * t5_pick<D>(z, a.cc_acomp);
-#pragma unroll
-                    for (int q = 0; q < P; q++) if (q == a.cc_aparam) {
-                        if (SA == SA_INTERP || SA == SA_BACKSOLVE) z[D + (L > D ? q : 0)] += gadd; else acc[q] += gadd;
-                    }
-                }
-                if (a.cc_lparam >= 0) {      // g = u_i - level - lcoef p[lparam]: -(dg/dp) w / (dg/du . f-)
-                    const double glev = a.cc_lcoef * corr;
-#pragma unroll
-                    for (int q = 0; q < P; q++) if (q == a.cc_lparam) {
-                        if (SA == SA_INTERP || SA == SA_BACKSOLVE) z[D + (L > D ? q : 0)] += glev; else acc[q] += glev;
-                    }
-                }
-#pragma unroll
-                for (int j = 0; j < D; j++) { z[j] *= sc[j]; if (j == a.cc_idx) z[j] -= corr; }
                 if (SA == SA_BACKSOLVE) {
 #pragma unroll
                     for (int j = 0; j < D; j++) z[YO + j] = um[j];

@@ -152,7 +152,9 @@ def _ball_inputs(N, shared_p, seed=3):
 @pytest.mark.parametrize("shared_p", [True, False])
 @pytest.mark.parametrize("sa", SENSEALGS)
 def test_ball_events_family_path_equals_the_named_path(families, sa, shared_p):
-    """BallEvents carries the built-in ball's named callback as family conditions: same events, same primal, same gradients."""
+    """BallEvents carries the built-in ball's named callback as family conditions.  Both run the same event search and
+    saltation with operands equal value for value, so the forward outputs are bitwise equal.  The gradients agree to a few
+    ulps (1.2e-15 of the largest du0 with per-member p on an H100), not bitwise: the two kernels are compiled separately."""
     N = 48
     u0, p = _ball_inputs(N, shared_p)
     t = np.linspace(0.5, 15.0, 30)
@@ -163,13 +165,12 @@ def test_ball_events_family_path_equals_the_named_path(families, sa, shared_p):
                   shared_p=shared_p, cost=b.AffineCost(1.0, 0.0), every=every)
     s1, st1 = named.forward(u0, p); g1 = named.reverse(); c1, t1 = named.event_times()
     s2, st2 = fam.forward(u0, p); g2 = fam.reverse(); c2, t2 = fam.event_times()
-    assert (np.asarray(st1) == 0).all() and (np.asarray(st2) == 0).all()
+    assert (np.asarray(st1) == 0).all() and np.array_equal(np.asarray(st1), np.asarray(st2))
     assert np.array_equal(c1, c2) and c1.min() >= 3
     mask = np.arange(t1.shape[0])[:, None] < c1[None, :]
-    bitwise = np.array_equal(t1[mask], t2[mask]) and np.array_equal(np.asarray(s1), np.asarray(s2))
-    print(f"{sa} shared_p={shared_p}: event times and saved bitwise equal: {bitwise}")
-    assert _rel(t2[mask], t1[mask]) < 1e-14 and _rel(s2, s1) < 1e-14
-    assert _rel(g2[0], g1[0]) < 1e-12 and _rel(g2[1], g1[1]) < 1e-12
+    assert np.array_equal(t1[mask], t2[mask]) and np.array_equal(np.asarray(s1), np.asarray(s2))
+    print(f"{sa} shared_p={shared_p}: du0 rel {_rel(g2[0], g1[0]):.1e}, dp rel {_rel(g2[1], g1[1]):.1e}")
+    assert _rel(g2[0], g1[0]) < 2e-15 and _rel(g2[1], g1[1]) < 2e-15
     flags = fam.event_flags()
     assert flags.shape == (32, 1, N) and (flags[:, 0][mask] == -1).all() and (flags[:, 0][~mask] == 0).all()
     cfg = O.make_cfg("ball", sa, "tsit5_adaptive", N, t, 0.0, 15.0, cost=("affine", 1.0, 0.0), shared_p=shared_p, ckpt_every_step=every,
