@@ -15,7 +15,7 @@ from .problems import (EM, AffineCost, ContinuousCallback, VectorContinuousCallb
                        Rosenbrock23, SDEProblem, Tsit5, saveat_to_times)
 from .sensitivity_algorithms import (B200Adjoint, BacksolveAdjoint, GaussAdjoint, GaussKronrodAdjoint, InterpolatingAdjoint,
                                      QuadratureAdjoint, sensealg_name)
-from .sensitivity_interface import _check_params, adjoint_sensitivities
+from .sensitivity_interface import _check_noise_mixing, _check_params, adjoint_sensitivities
 
 
 class NoTangent:
@@ -113,6 +113,7 @@ def solve(eprob, alg, ensemblealg=None, *, trajectories=None, saveat=None, sense
     if prob.f not in FAMILIES:
         raise KeyError(f"unknown RHS family {prob.f!r}; known: {sorted(FAMILIES)}")
     d, P, m = FAMILIES[prob.f]
+    _check_noise_mixing(prob.f, sensealg)
     if u0 is None or p is None:
         if trajectories is None:
             trajectories = eprob.u0s.shape[1] if eprob.u0s is not None else 1

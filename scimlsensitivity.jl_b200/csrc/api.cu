@@ -36,27 +36,34 @@ FamilyVTable builtin_family(const char* name) {
     if constexpr (F32) { v.fwd_f32 = &launch_fwd_f32<F>; v.rev_f32 = &launch_rev_f32<F>; }
     return v;
 }
+// a built-in diagonal-noise SDE family: the EM / EulerHeun launchers disp_sde.cu instantiates
+template <template <bool> class F>
+FamilyVTable builtin_sde_family(const char* name) {
+    FamilyVTable v = {B200ADJ_PLUGIN_ABI, F<false>::D, F<false>::P, name};
+    v.m = F<false>::M; v.sde_fwd = &launch_sde_fwd<F>; v.sde_rev = &launch_sde_rev<F>;
+    return v;
+}
 constexpr int BUILTIN_FAMILIES = B200ADJ_FAM_RELAX + 1;
-const FamilyVTable* builtin_families() {        // indexed by B200ADJ_FAM_*; abi == 0: an SDE / MLP family (own dispatch)
+const FamilyVTable* builtin_families() {        // indexed by B200ADJ_FAM_*; abi == 0: the MLP family (own dispatch)
     static const FamilyVTable t[BUILTIN_FAMILIES] = {
         builtin_family<LotkaVolterra, true, true, true>("lv"),
         builtin_family<Lorenz, true, true, true>("lorenz"),
         builtin_family<Robertson, true, true, false>("robertson"),
-        {}, {}, {},                             // SDE_LV, MLP, SDE_LINEAR
+        builtin_sde_family<SdeLotkaVolterra>("sde_lv"),
+        {},                                     // MLP
+        builtin_sde_family<SdeLinear2>("sde_linear"),
         builtin_family<BouncingBall, false, false, false>("ball"),
         builtin_family<Relax, false, false, false>("relax")};
     return t;
 }
 
-// d, P, m of the families with their own dispatch entry points (sde_*_dispatch, mlp_*_dispatch)
+// d, P, m of the families with their own dispatch entry points (mlp_*_dispatch)
 struct FamDims { int32_t id, d, P, m; };
 constexpr FamDims OWN_DISPATCH_FAMILIES[] = {
-    {B200ADJ_FAM_SDE_LV, SdeLotkaVolterra<false>::D, SdeLotkaVolterra<false>::P, SdeLotkaVolterra<false>::M},
-    {B200ADJ_FAM_SDE_LINEAR, SdeLinear2<false>::D, SdeLinear2<false>::P, SdeLinear2<false>::M},
     {B200ADJ_FAM_MLP, MLP_D, MLP_P, 0}};
 
 int fam_dims(const b200adj_cfg& c, int* d, int* P, int* m) {
-    if (const FamilyVTable* vt = family_lookup(c.rhs_family)) { *d = vt->d; *P = vt->P; *m = 0; return 0; }
+    if (const FamilyVTable* vt = family_lookup(c.rhs_family)) { *d = vt->d; *P = vt->P; *m = vt->m; return 0; }
     if (c.rhs_family == B200ADJ_FAM_MLP && c.mlp_hidden != MLP_H) return -1;
     for (const FamDims& f : OWN_DISPATCH_FAMILIES)
         if (f.id == c.rhs_family) { *d = f.d; *P = f.P; *m = f.m; return 0; }
@@ -561,6 +568,8 @@ int32_t b200adj_register_family(const char* plugin_path, int32_t* family_id) {
     // a refused plug-in is unloaded again, so that a rebuilt file of the same name is really loaded next time
     if (!vt || vt->abi != B200ADJ_PLUGIN_ABI) { dlclose(lib); g_create_error = "register_family: plug-in built against other headers (ABI tag mismatch): rebuild it"; return B200ADJ_ERR_INVALID; }
     if (vt->d < 1 || vt->d > 4 || vt->P < 1 || vt->P > 8) { dlclose(lib); g_create_error = "register_family: 1 <= D <= 4 and 1 <= P <= 8"; return B200ADJ_ERR_UNSUPPORTED; }
+    if (vt->m != 0 && (vt->m != vt->d || !vt->sde_fwd || !vt->sde_rev)) {
+        dlclose(lib); g_create_error = "register_family: an SDE plug-in has diagonal noise (M == D) and the EM / EulerHeun launchers"; return B200ADJ_ERR_UNSUPPORTED; }
     auto& r = family_registry();
     for (size_t k = 0; k < r.size(); k++) if (r[k] == vt) { *family_id = B200ADJ_FAM_USER_BASE_ID + (int)k; return B200ADJ_OK; }
     r.push_back(vt);
@@ -741,6 +750,14 @@ int32_t b200adj_family_conditions(int32_t family, int32_t* nc) {
     return B200ADJ_ERR_INVALID;
 }
 
+int32_t b200adj_family_noise(int32_t family, int32_t* m) {
+    if (!m) return B200ADJ_ERR_INVALID;
+    if (const FamilyVTable* vt = family_lookup(family)) { *m = vt->m; return B200ADJ_OK; }
+    for (const FamDims& f : OWN_DISPATCH_FAMILIES)
+        if (f.id == family) { *m = f.m; return B200ADJ_OK; }
+    return B200ADJ_ERR_INVALID;
+}
+
 int32_t b200adj_set_family_events(void* handle, int32_t enabled, int32_t nc, const int32_t* direction, int32_t max_events) {
     if (!handle) return B200ADJ_ERR_INVALID;
     Handle* h = (Handle*)handle;
@@ -831,7 +848,7 @@ int32_t b200adj_forward(void* handle, const void* u0, const void* p, const void*
         dstatus = status ? h->s_status : nullptr;
     }
     h->cur_p = dp;
-    const FamilyVTable* vt = family_lookup(c.rhs_family);      // the ODE paths' launchers
+    const FamilyVTable* vt = family_lookup(c.rhs_family);      // the ODE and SDE paths' launchers
     int rc = 0;
     if (is_adaptive(h)) {
         auto fwd = [&](auto a, auto fn, int32_t* st) {
@@ -878,7 +895,7 @@ int32_t b200adj_forward(void* handle, const void* u0, const void* p, const void*
         } else {
             h->noise_valid = false;
         }
-        rc = sde_forward_dispatch(h, a);
+        rc = launch(vt->sde_fwd, h, a);
     }
     if (rc) { h->err = "forward dispatch failed"; return rc; }
     CUDA_TRY(h, cudaGetLastError());
@@ -912,7 +929,7 @@ int32_t b200adj_reverse(void* handle, const void* dLdu, void* du0, void* dp) {
     }
     int rc = 0;
     bool fused_allreduce = false;
-    const FamilyVTable* vt = family_lookup(c.rhs_family);      // the ODE paths' launchers
+    const FamilyVTable* vt = family_lookup(c.rhs_family);      // the ODE and SDE paths' launchers
     if (is_adaptive(h)) {
         auto rev = [&](auto a, auto fn) {
             a.p = h->cur_p; a.dLdu = dL; a.du0 = ddu0; a.dp_members = ddp; a.dp = ddp;
@@ -962,7 +979,7 @@ int32_t b200adj_reverse(void* handle, const void* dLdu, void* du0, void* dp) {
         a.flags = kernel_flags(h);
         a.seed = c.seed; a.traj_offset = c.traj_offset;
         a.noise = h->noise_valid ? h->d_noise : nullptr;
-        rc = sde_reverse_dispatch(h, a);
+        rc = launch(vt->sde_rev, h, a);
     }
     if (rc) { h->err = "reverse dispatch failed (sensealg/family not built)"; return rc; }
     CUDA_TRY(h, cudaGetLastError());

@@ -1,57 +1,11 @@
-// disp_sde.cu -- launchers of the SDE kernels (sde_em.cuh): EM / EulerHeun forward, Backsolve / Interpolating reverse
-#include "handle.h"
+// disp_sde.cu -- SDE kernels (disp_sde.inc) instantiated for the built-in families SdeLotkaVolterra and SdeLinear2, and
+// the noise export kernel
+#include "disp_sde.inc"
 namespace b200adj {
-namespace {
-template <class Fam, bool EH>
-int launch_sde_fwd_f(Handle* h, const SdeFwdArgs& a) {
-    if (h->cfg.shared_p) sde_forward_kernel<Fam, EH, true><<<h->grid, h->block, 0, h->stream>>>(a);
-    else sde_forward_kernel<Fam, EH, false><<<h->grid, h->block, 0, h->stream>>>(a);
-    h->launches++;
-    return 0;
-}
-template <class Fam, bool EH, bool SHARED_P, int COST, bool INTERP>
-int launch_sde_rev_b(Handle* h, const SdeRevArgs& a) {
-    sde_backsolve_kernel<Fam, EH, SHARED_P, COST, INTERP><<<h->grid, h->block, 0, h->stream>>>(a);
-    h->launches++;
-    return 0;
-}
-template <class Fam, bool EH, bool INTERP>
-int launch_sde_rev_f(Handle* h, const SdeRevArgs& a) {
-    const bool sp = h->cfg.shared_p;
-    const bool ex = h->cfg.cost_kind == B200ADJ_COST_EXPLICIT;
-    if (sp) return ex ? launch_sde_rev_b<Fam, EH, true, COST_EXPLICIT, INTERP>(h, a) : launch_sde_rev_b<Fam, EH, true, COST_AFFINE, INTERP>(h, a);
-    return ex ? launch_sde_rev_b<Fam, EH, false, COST_EXPLICIT, INTERP>(h, a) : launch_sde_rev_b<Fam, EH, false, COST_AFFINE, INTERP>(h, a);
-}
-}  // namespace
-
-int sde_forward_dispatch(Handle* h, const SdeFwdArgs& a) {
-    const b200adj_cfg& c = h->cfg;
-    const bool eh = c.stepper == B200ADJ_ST_EULER_HEUN;
-    switch (c.rhs_family) {
-    case B200ADJ_FAM_SDE_LV: return eh ? launch_sde_fwd_f<SdeLotkaVolterra<false>, true>(h, a) : launch_sde_fwd_f<SdeLotkaVolterra<false>, false>(h, a);
-    case B200ADJ_FAM_SDE_LINEAR: return eh ? launch_sde_fwd_f<SdeLinear2<false>, true>(h, a) : launch_sde_fwd_f<SdeLinear2<false>, false>(h, a);
-    default: return B200ADJ_ERR_UNSUPPORTED;
-    }
-}
-
-int sde_reverse_dispatch(Handle* h, const SdeRevArgs& a) {
-    const b200adj_cfg& c = h->cfg;
-    const bool eh = c.stepper == B200ADJ_ST_EULER_HEUN;
-    const bool interp = c.sensealg == B200ADJ_SA_INTERPOLATING;
-    // Backsolve + Ito solver (EM): transformed drift; InterpolatingAdjoint: the problem's own drift
-    if (interp) {
-        switch (c.rhs_family) {
-        case B200ADJ_FAM_SDE_LV: return eh ? launch_sde_rev_f<SdeLotkaVolterra<false>, true, true>(h, a) : launch_sde_rev_f<SdeLotkaVolterra<false>, false, true>(h, a);
-        case B200ADJ_FAM_SDE_LINEAR: return eh ? launch_sde_rev_f<SdeLinear2<false>, true, true>(h, a) : launch_sde_rev_f<SdeLinear2<false>, false, true>(h, a);
-        default: return B200ADJ_ERR_UNSUPPORTED;
-        }
-    }
-    switch (c.rhs_family) {
-    case B200ADJ_FAM_SDE_LV: return eh ? launch_sde_rev_f<SdeLotkaVolterra<false>, true, false>(h, a) : launch_sde_rev_f<SdeLotkaVolterra<true>, false, false>(h, a);
-    case B200ADJ_FAM_SDE_LINEAR: return eh ? launch_sde_rev_f<SdeLinear2<false>, true, false>(h, a) : launch_sde_rev_f<SdeLinear2<true>, false, false>(h, a);
-    default: return B200ADJ_ERR_UNSUPPORTED;
-    }
-}
+template int launch_sde_fwd<SdeLotkaVolterra>(Handle*, const SdeFwdArgs&);
+template int launch_sde_rev<SdeLotkaVolterra>(Handle*, const SdeRevArgs&);
+template int launch_sde_fwd<SdeLinear2>(Handle*, const SdeFwdArgs&);
+template int launch_sde_rev<SdeLinear2>(Handle*, const SdeRevArgs&);
 
 int sde_noise_launch(Handle* h, const SdeNoiseArgs& a, int64_t total) {
     sde_noise_kernel<0><<<(unsigned)((total + 255) / 256), 256, 0, h->stream>>>(a);

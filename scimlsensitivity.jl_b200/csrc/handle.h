@@ -139,9 +139,11 @@ template <class T, class S> inline void cast_tables(const S& src, T* dst) {
 
 // ---- family registry (SURVEY.md 8f rank 4; the seam user-supplied ODEFunction(f; vjp, vjp_p, jac, paramjac) occupies in the
 // reference, src/derivative_wrappers.jl:284-359, test/Core3/user_vjp.jl:14-38).  A family PLUG-IN is a shared library built from
-// a user header that defines one struct with the shape of families.cuh (D, P, f, vjp_u, vjp_p [, jac, djac, dvjp_p]); the
-// plug-in instantiates the same kernel templates for it and exports this table of launchers (family_plugin.inc).
-// b200adj_register_family(path) loads it and hands out a family id >= B200ADJ_FAM_USER_BASE. ----
+// a user header that defines one struct with the shape of families.cuh (D, P, f, vjp_u, vjp_p [, jac, djac, dvjp_p]), or for a
+// diagonal-noise SDE one `template <bool ITO> struct` with the shape of SdeLotkaVolterra (D, P, M = D, f, g and their VJPs);
+// the plug-in instantiates the same kernel templates for it and exports this table of launchers (family_plugin.inc).
+// b200adj_register_family(path) loads it and hands out a family id >= B200ADJ_FAM_USER_BASE.  The built-in families fill
+// the same table (api.cu, builtin_families), so every family but MLP dispatches through one lookup. ----
 struct FamilyVTable {
     uint32_t abi;                 // B200ADJ_PLUGIN_ABI of the headers the plug-in was built from
     int32_t d, P;
@@ -155,11 +157,15 @@ struct FamilyVTable {
     int (*fwd_f32)(Handle*, const OdeFwdArgsT<float>&);     // fixed-step Tsit5 in F32 (built-in LV / Lorenz; null elsewhere)
     int (*rev_f32)(Handle*, const OdeRevArgsT<float>&);
     int32_t nc;                   // conditions of the family's own state-dependent event (B200ADJ_FAMILY_HAS_EVENTS); 0: none
+    int32_t m;                    // Wiener processes of an SDE family (diagonal noise: m = d); 0: an ODE family
+    int (*sde_fwd)(Handle*, const SdeFwdArgs&);      // EM / EulerHeun (SDE families only; null for an ODE family)
+    int (*sde_rev)(Handle*, const SdeRevArgs&);
 };
 constexpr uint32_t B200ADJ_PLUGIN_ABI = 0x00020000u ^ (uint32_t)sizeof(Handle) ^ ((uint32_t)sizeof(OdeRevArgs) << 8) ^
-                                        ((uint32_t)sizeof(T5aArgs) << 16) ^ ((uint32_t)sizeof(FamilyVTable) << 24);
+                                        ((uint32_t)sizeof(T5aArgs) << 16) ^ ((uint32_t)sizeof(FamilyVTable) << 24) ^
+                                        ((uint32_t)sizeof(SdeFwdArgs) << 4) ^ ((uint32_t)sizeof(SdeRevArgs) << 12);
 constexpr int B200ADJ_FAM_USER_BASE_ID = 100;
-// api.cu: the ODE families, built-in (id < B200ADJ_FAM_USER_BASE_ID) and registered plug-ins; null for the SDE / MLP families
+// api.cu: the ODE and SDE families, built-in (id < B200ADJ_FAM_USER_BASE_ID) and registered plug-ins; null for the MLP family
 const FamilyVTable* family_lookup(int id);
 
 // ---- dispatch entry points, one explicit instantiation per family in disp_*.cu ----
@@ -171,8 +177,8 @@ template <class Fam> int launch_t5a_fwd(Handle* h, const T5aArgs& a);
 template <class Fam> int launch_t5a_rev(Handle* h, const T5aArgs& a);
 template <class Fam> int launch_ros_fwd(Handle* h, const RosArgs& a);
 template <class Fam> int launch_ros_rev(Handle* h, const RosArgs& a);
-int sde_forward_dispatch(Handle* h, const SdeFwdArgs& a);
-int sde_reverse_dispatch(Handle* h, const SdeRevArgs& a);
+template <template <bool> class Fam> int launch_sde_fwd(Handle* h, const SdeFwdArgs& a);     // disp_sde.inc
+template <template <bool> class Fam> int launch_sde_rev(Handle* h, const SdeRevArgs& a);
 int sde_noise_launch(Handle* h, const SdeNoiseArgs& a, int64_t total);
 int mlp_forward_dispatch(Handle* h, const void* u0, const void* p, void* saved, int32_t* status);
 int mlp_reverse_dispatch(Handle* h, const void* dLdu, void* du0, void* dp);

@@ -7,7 +7,13 @@ event: NC, condition, condition_grad, affect, affect_vjp -- csrc/family_plugin.i
 instantiates the library's own kernel templates for it -- no .cu file of the library is edited) and `register_family` it; the
 name is then usable wherever "lv" / "lorenz" are.
 
+A diagonal-noise SDE family (`sde=True`, `--sde`) is ONE `template <bool ITO> struct` with the shape of SdeLotkaVolterra in
+csrc/families.cuh: D, P, M = D, the drift f with vjp_u / vjp_p (with ITO = true: the Ito-transformed drift f - (dg/du)' g and
+its VJPs), the diffusion g with gvjp_u / gvjp_p_apply, where g_i depends on u_i and p only (noisemixing = false).  Its name is
+then usable wherever "sde_lv" is: SDEProblem with EM / EulerHeun and BacksolveAdjoint / InterpolatingAdjoint.
+
     python -m scimlsensitivity_jl_b200.family_plugin my_family.cuh VanDerPol vanderpol [--jac] [--events] [-o libfam_vanderpol.so]
+    python -m scimlsensitivity_jl_b200.family_plugin my_sde.cuh MySde my_sde --sde
 """
 import ctypes as C
 import os
@@ -19,9 +25,12 @@ from . import _lib
 from .problems import FAMILIES, FAMILY_CONDITIONS
 
 
-def build_family_plugin(header, struct, name, out=None, has_jac=False, verbose=False, has_events=False):
+def build_family_plugin(header, struct, name, out=None, has_jac=False, verbose=False, has_events=False, sde=False):
     """Compile `struct` of the CUDA header `header` into a family plug-in (shared library); returns its path.
-    has_events: the struct carries NC conditions and their affect (VectorContinuousCallback on the adaptive Tsit5 path)."""
+    has_events: the struct carries NC conditions and their affect (VectorContinuousCallback on the adaptive Tsit5 path).
+    sde: `struct` is a `template <bool ITO> struct` of a diagonal-noise SDE family (EM / EulerHeun kernels only)."""
+    if sde and (has_jac or has_events):
+        raise ValueError("an SDE family plug-in carries the EM / EulerHeun kernels only (no jac, no events)")
     header = os.path.abspath(header)
     out = os.path.abspath(out or os.path.join(os.path.dirname(header), f"libb200fam_{name}.so"))
     if os.path.exists(out) and os.path.getmtime(out) >= max(os.path.getmtime(header), os.path.getmtime(_lib.LIB_PATH)):
@@ -35,6 +44,8 @@ def build_family_plugin(header, struct, name, out=None, has_jac=False, verbose=F
                 f.write("#define B200ADJ_FAMILY_HAS_JAC 1\n")
             if has_events:
                 f.write("#define B200ADJ_FAMILY_HAS_EVENTS 1\n")
+            if sde:
+                f.write("#define B200ADJ_FAMILY_SDE 1\n")
             f.write('#include "family_plugin.inc"\n')
         cmd = [_lib.nvcc_path(), "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC",
                "-shared", "-I", _lib._CSRC, src, "-o", out, "-L", pkg, "-l:" + os.path.basename(_lib.LIB_PATH), "-Xlinker", "-rpath", "-Xlinker", pkg]
@@ -57,7 +68,7 @@ def register_family(plugin_path, name=None):
     lib.b200adj_family_info(fid.value, C.byref(d), C.byref(P), C.byref(nm))
     name = name or nm.value.decode()
     _lib.FAM[name] = fid.value
-    FAMILIES[name] = (d.value, P.value, 0)
+    FAMILIES[name] = (d.value, P.value, _lib.family_noise(fid.value))
     FAMILY_CONDITIONS[name] = _lib.family_conditions(fid.value)
     return fid.value, d.value, P.value
 
@@ -69,6 +80,8 @@ if __name__ == "__main__":
     ap.add_argument("--jac", action="store_true", help="the struct also has jac / djac / dvjp_p: build the Rosenbrock23 kernels")
     ap.add_argument("--events", action="store_true", help="the struct also has NC / condition / condition_grad / affect / affect_vjp: "
                     "build the kernels of its state-dependent event")
+    ap.add_argument("--sde", action="store_true", help="the struct is a `template <bool ITO> struct` of a diagonal-noise SDE family: "
+                    "build the EM / EulerHeun kernels")
     ap.add_argument("-o", "--out", default=None)
     a = ap.parse_args()
-    print(build_family_plugin(a.header, a.struct, a.name, a.out, a.jac, verbose=True, has_events=a.events))
+    print(build_family_plugin(a.header, a.struct, a.name, a.out, a.jac, verbose=True, has_events=a.events, sde=a.sde))

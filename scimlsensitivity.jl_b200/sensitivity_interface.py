@@ -8,9 +8,22 @@ src/sensitivity_interface.jl:503-507).  For an ensemble `du0` is [d, N]; with pe
 """
 import numpy as np
 
-from .problems import AdjointSensitivityParameterCompatibilityError, AffineCost, ParamAffine, QuadraticRunningCost
+from . import _lib
+from .problems import FAMILIES, AdjointSensitivityParameterCompatibilityError, AffineCost, ParamAffine, QuadraticRunningCost
 from .sensitivity_algorithms import (B200Adjoint, BacksolveAdjoint, GaussAdjoint, GaussKronrodAdjoint, InterpolatingAdjoint,
-                                     QuadratureAdjoint, sensealg_name)
+                                     QuadratureAdjoint, isnoisemixing, sensealg_name)
+
+FAM_USER_BASE = 100      # B200ADJ_FAM_USER_BASE: ids of registered plug-in families
+
+
+def _check_noise_mixing(family, sensealg):
+    """A plug-in SDE family's kernels take g_i to depend on u_i and p only (csrc/family_plugin.inc): the noisemixing = true
+    diffusion VJP of the reference (src/derivative_wrappers.jl:1165-1211) is not built for it."""
+    if sensealg is None or not isnoisemixing(sensealg):
+        return
+    if FAMILIES.get(family, (0, 0, 0))[2] and _lib.FAM.get(family, -1) >= FAM_USER_BASE:
+        raise NotImplementedError(f"noisemixing = true: the SDE family plug-in {family!r} is built for diagonal noise that does not "
+                                  "mix (g_i depends on u_i and p only)")
 
 
 def _check_params(p):
@@ -76,6 +89,7 @@ def adjoint_sensitivities(sol, alg=None, *, sensealg=None, t=None, dgdu_discrete
     eng = sol.engine
     if eng is None:
         raise RuntimeError("solution carries no live device handle")
+    _check_noise_mixing(eng.family, sensealg)
     ts = sol.t if t is None else np.asarray(t, dtype=np.float64)
     if dgdu_discrete is None:
         ts = np.zeros(0)                                   # continuous cost only: no jumps (discrete = false in the reference)
