@@ -82,8 +82,11 @@ class Kind:
 
 
 def vjp(kind, f, y, p, l, wrt):
-    """(df/du)' l (wrt = 'u') or (df/dp)' l (wrt = 'p') by complex steps of l' f(y, p); y, p, l lists of member arrays"""
-    yc, pc = [kind.cplx(v) for v in y], [kind.cplx(v) for v in p]
+    """(df/du)' l (wrt = 'u') or (df/dp)' l (wrt = 'p') by complex steps of l' f(y, p); y, p, l lists of member arrays.
+    A family with many parameters supplies (df/dp)' l itself, as f.vjp_p(kind, y, p, l) -> one [P][M] array"""
+    if wrt == "p" and hasattr(f, "vjp_p"):
+        return f.vjp_p(kind, y, p, l)
+    yc, pc = [kind.cplx(v) for v in y], ([kind.cplx(v) for v in p] if wrt == "p" else p)
     out = []
     for c in range(len(y) if wrt == "u" else len(p)):
         yy, pp = list(yc), list(pc)
@@ -115,19 +118,27 @@ def lin(a, xs, ws):
     return [a[c] + sum(w * x[c] for w, x in zip(ws, xs)) for c in range(len(a))]
 
 
+def axpy(mu, w, g):
+    """mu + w g over the parameters: g a list of member arrays, or one [P][M] array from a family's vjp_p"""
+    if isinstance(g, np.ndarray) and g.ndim == 2:
+        return np.asarray(mu) + w * g
+    return [mu[q] + w * g[q] for q in range(len(mu))]
+
+
 class Problem:
-    """one fixed-grid problem: family, h, S, u0[D][M], per-member p[P][M], save table {n: k}, cost, events
-    {n: (s, c, ps, pc)}, continuous cost (a, b) or None, no_start"""
+    """one fixed-grid problem: family (a name of FAMS or a triple (f, D, P)), h, S, u0[D][M], per-member p[P][M], save
+    table {n: k}, cost ('explicit' or (a, b), scalars or per-component vectors), events {n: (s, c, ps, pc)}, continuous
+    cost (a, b) or None, no_start"""
 
     def __init__(self, family, h, S, u0, p, sos, cost, dLdu=None, events=None, cont=None, no_start=False):
-        self.f, self.D, self.P = FAMS[family]
+        self.f, self.D, self.P = FAMS[family] if isinstance(family, str) else family
         self.h, self.S, self.u0, self.p, self.sos, self.cost, self.dLdu = h, S, u0, p, sos, cost, dLdu
         self.events, self.cont, self.no_start = events or {}, cont, no_start
 
 
 def params_of(kind, pr, n):
     """parameters in force on step n (after the events at grid points <= n)"""
-    p = [kind.arr(q) for q in pr.p]
+    p = kind.arr(pr.p)
     for m in sorted(pr.events):
         if m > n:
             break
@@ -170,8 +181,8 @@ def jump(kind, pr, n, y):
         return None
     if pr.cost == "explicit":
         return [kind.arr(pr.dLdu[pr.sos[n], c]) for c in range(pr.D)]
-    a, b = pr.cost
-    return [kind.const(a) * y[c] + kind.const(b) for c in range(pr.D)]
+    a, b = (np.broadcast_to(np.asarray(v, dtype=np.float64), (pr.D,)) for v in pr.cost)
+    return [kind.const(a[c]) * y[c] + kind.const(b[c]) for c in range(pr.D)]
 
 
 def add_cont(kind, pr, y, ka):
@@ -204,8 +215,9 @@ def _gl(n):
     return xs, ws
 
 
-def reverse(kind, tab, pr, sensealg, us, Ks, ps, gk_log=None, ckpt_mode="save"):
-    """-> (du0[D][M], dp[P][M]) of the restatement"""
+def reverse(kind, tab, pr, sensealg, us, Ks, ps, gk_log=None, ckpt_mode="save", gauss_y=None):
+    """-> (du0[D][M], dp[P][M]) of the restatement; gauss_y(tha) -> the forward dense output's theta at a Gauss node
+    (1 - tha; other maps restate a wrong kernel)"""
     f, D, P = pr.f, pr.D, pr.P
     h = kind.const(pr.h)
     M = len(us[0][0])
@@ -229,18 +241,18 @@ def reverse(kind, tab, pr, sensealg, us, Ks, ps, gk_log=None, ckpt_mode="save"):
         if sensealg == "interpolating":
             for s in range(6):
                 g = vjp(kind, f, ys[s], p, ls[s], "p")
-                mu = [mu[q] + h * tab.A[6][s] * g[q] for q in range(P)]
+                mu = axpy(mu, h * tab.A[6][s], g)
         else:
             def node(tha):
                 """integrand at time t_{n+1} - tha h: (df/dp)' lambda, lambda from the adjoint step's dense output"""
                 lq = dense(kind, tab, h, lam, ka, tha)
-                yq = dense(kind, tab, h, un, k, 1 - Fraction(tha) if not isinstance(tha, mp.mpf) else 1 - tha)
+                yq = dense(kind, tab, h, un, k, gauss_y(tha) if gauss_y else 1 - Fraction(tha) if not isinstance(tha, mp.mpf) else 1 - tha)
                 return vjp(kind, f, yq, p, lq, "p")
             if sensealg == "gauss":
                 a = Fraction(1, 2) * (1 - Fraction(mp.nstr(mp.sqrt(mp.mpf("0.6")), 45)))
                 for tha, w in ((a, Fraction(5, 9)), (Fraction(1, 2), Fraction(8, 9)), (1 - a, Fraction(5, 9))):
                     g = node(tha)
-                    mu = [mu[q] + h / 2 * kind.const(w) * g[q] for q in range(P)]
+                    mu = axpy(mu, h / 2 * kind.const(w), g)
             elif sensealg == "quadrature":
                 global GL8
                 if GL8 is None:
