@@ -158,6 +158,15 @@ void tsit5_weights(double th, double* w, double (*Rout)[4]) {
     if (w) for (int j = 0; j < 7; j++) w[j] = (((R[j][4] * th + R[j][3]) * th + R[j][2]) * th + R[j][1]) * th + R[j][0];
 }
 
+// The 7 points of the Hermite-form dense output (ode_tsit5.cuh, tsit5_dense_hermite): the 4 stage times of hBst, then the
+// y-side Gauss nodes, the theta of hBq[2 - g] at row 4 + g
+void hermite_thetas(double* th) {
+    const double a = sqrt(0.6);
+    const double thq[3] = {0.5 * (1.0 - a), 0.5, 0.5 * (1.0 + a)};
+    for (int s = 1; s <= 4; s++) th[s - 1] = 1.0 - TSIT5_C[s];
+    for (int g = 0; g < 3; g++) th[4 + g] = thq[2 - g];
+}
+
 // Step-size-scaled Tsit5 tables for one handle (passed to the kernels by value, i.e. through the constant bank).
 void build_tsit5_tables(double h, Tsit5Tables* t) {
     const double (&A)[7][6] = TSIT5_A;
@@ -170,8 +179,10 @@ void build_tsit5_tables(double h, Tsit5Tables* t) {
     const double thq[3] = {0.5 * (1.0 - a), 0.5, 0.5 * (1.0 + a)};
     for (int g = 0; g < 3; g++) { tsit5_weights(thq[g], w); for (int j = 0; j < 7; j++) t->hBq[g][j] = h * w[j]; }
     t->hGW[0] = 0.5 * h * (5.0 / 9.0); t->hGW[1] = 0.5 * h * (8.0 / 9.0); t->hGW[2] = 0.5 * h * (5.0 / 9.0);
-    // Hermite form (ode_tsit5.cuh, tsit5_dense_hermite): the 4 stage times of hBst, then the y-side Gauss nodes hBq[2 - g]
-    const double thh[7] = {1.0 - C[1], 1.0 - C[2], 1.0 - C[3], 1.0 - C[4], thq[2], thq[1], thq[0]};
+    // Hermite form {H01, h H10, h H11, theta^2 (1-theta)^2} at the points of hermite_thetas (the kernels read the folded
+    // rows of build_hermite_folded)
+    double thh[7];
+    hermite_thetas(thh);
     for (int r = 0; r < 7; r++) {
         const double x = thh[r], x2 = x * x, x3 = x2 * x;
         t->hHm[r][0] = 3.0 * x2 - 2.0 * x3;
@@ -193,6 +204,28 @@ void build_c4_du_weights(double h, double* w) {
     for (int j = 0; j < 5; j++) w[j] = (double)((LD)h * ((LD)R[j][3] - r6 * (LD)TSIT5_A[6][j] / b6));
     w[5] = (double)(r6 / b6);
     w[6] = h * R[6][3];
+}
+
+// The Hermite point table with the c4 elimination folded in (OdeRevArgsT::hHf; ode_tsit5.cuh, tsit5_dense_hermite).  With
+// c4 = w_0 k1 + sum_{j=1..4} w_j k_j + w_5 du + w_6 k7 (build_c4_du_weights) and G = theta^2 (1-theta)^2, the point
+//   u_n + H01 du + h H10 k1 + h H11 k7 + G c4  =  u_n + (H01 + G w_5) du + (h H10 + G w_0) k1 + (h H11 + G w_6) k7 + G c4''
+// with c4'' = sum_{j=1..4} w_j k_j.  Row r = {H01 + G w_5, h H10 + G w_0, h H11 + G w_6, G} at the theta of hHm[r].  In long
+// double from the Hermite polynomials and the unrounded w_0, w_5, w_6: the folded weights cancel (|G w_5| <= 15/16 against
+// H01 <= 1), and a double evaluation leaves them up to 24 ulps off (tests/test_tsit5_folded_tables.py).
+void build_hermite_folded(double h, double (*hf)[4]) {
+    typedef long double LD;
+    double R[7][4], th[7];
+    tsit5_weights(0.0, nullptr, R);
+    hermite_thetas(th);
+    const LD b6 = TSIT5_A[6][5], r6 = R[5][3], H = h;
+    const LD w0 = H * ((LD)R[0][3] - r6 * (LD)TSIT5_A[6][0] / b6), w5 = r6 / b6, w6 = H * (LD)R[6][3];
+    for (int r = 0; r < 7; r++) {
+        const LD x = th[r], x2 = x * x, x3 = x2 * x, G = x2 * (1 - x) * (1 - x);
+        hf[r][0] = (double)(3 * x2 - 2 * x3 + G * w5);
+        hf[r][1] = (double)(H * (x - 2 * x2 + x3) + G * w0);
+        hf[r][2] = (double)(H * (x3 - x2) + G * w6);
+        hf[r][3] = (double)G;
+    }
 }
 
 const FamilyVTable* family_lookup(int id) {
@@ -949,9 +982,7 @@ int32_t b200adj_reverse(void* handle, const void* dLdu, void* du0, void* dp) {
         a.N = c.N; a.Npad = h->Npad; a.S = h->S; a.trace = h->d_trace;
         for (int j = 0; j < 4; j++) { a.cost_a[j] = (float)h->cost_av[j]; a.cost_b[j] = (float)h->cost_bv[j]; }
         cast_tables(h->tb, &a.tb);
-        double w[7];
-        build_c4_du_weights(c.dt, w);
-        for (int j = 0; j < 7; j++) a.hC4u[j] = (float)w[j];
+        build_hermite_weights_f32(c.dt, a.hC4u, a.hHf);
         a.flags = kernel_flags(h);
         rc = launch(vt->rev_f32, h, a);
     } else if (h->path == Path::FIXED) {
@@ -960,6 +991,7 @@ int32_t b200adj_reverse(void* handle, const void* dLdu, void* du0, void* dp) {
         a.event_of_step = h->d_event_of_step; a.ev_s = h->d_ev_s; a.ev_c = h->d_ev_c; a.ev_ps = h->d_ev_ps; a.ev_pc = h->d_ev_pc; a.nev = h->nev;
         tsit5_weights(0.0, nullptr, a.Rpoly); a.hstep = c.dt;
         build_c4_du_weights(c.dt, a.hC4u);
+        build_hermite_folded(c.dt, a.hHf);
         if (c.shared_p && comm_fused_ready(h) && !(c.flags & B200ADJ_FLAG_NCCL_ALLREDUCE) && c.sensealg != B200ADJ_SA_QUADRATURE && !h->has_dgdp && !(h->has_cdgdp && h->cont_on)) {
             // the all-reduce of dp is fused into this kernel's last block (peer-memory mailboxes): no collective launch
             a.p2p = h->p2p; a.p2p.epoch = ++h->p2p_epoch; fused_allreduce = true;

@@ -127,6 +127,16 @@ inline size_t esz(const b200adj_cfg& c) { return c.dtype == B200ADJ_F64 ? sizeof
 void tsit5_weights(double th, double* w, double (*Rout)[4] = nullptr);
 void build_tsit5_tables(double h, Tsit5Tables* t);
 void build_c4_du_weights(double h, double* w);     // OdeRevArgsT::hC4u
+void hermite_thetas(double* th);                   // the 7 theta of Tsit5Tables::hHm and OdeRevArgsT::hHf
+void build_hermite_folded(double h, double (*hf)[4]);   // OdeRevArgsT::hHf
+// OdeRevArgsT<float>::hC4u and hHf: the fp64 weights, each rounded once to float
+inline void build_hermite_weights_f32(double h, float* c4u, float (*hf)[4]) {
+    double w[7], f[7][4];
+    build_c4_du_weights(h, w);
+    build_hermite_folded(h, f);
+    for (int j = 0; j < 7; j++) c4u[j] = (float)w[j];
+    for (int r = 0; r < 7; r++) for (int j = 0; j < 4; j++) hf[r][j] = (float)f[r][j];
+}
 template <class T, class S> inline void cast_tables(const S& src, T* dst) {
     for (int i = 0; i < 7; i++) for (int j = 0; j < 6; j++) dst->hA[i][j] = (float)src.hA[i][j];
     for (int i = 0; i < 4; i++) for (int j = 0; j < 7; j++) dst->hBst[i][j] = (float)src.hBst[i][j];

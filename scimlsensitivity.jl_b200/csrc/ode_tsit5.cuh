@@ -34,9 +34,10 @@ template <class R> struct Tsit5TablesT {
     R hBst[4][7];  // h * b_j(theta) at theta = 1 - c_s for adjoint stages s = 1..4 (0-based)
     R hBq[3][7];   // h * b_j(theta) at theta = (1 -/+ sqrt(.6))/2, 1/2  (3-pt Gauss-Legendre nodes)
     R hGW[3];      // (h/2) * Gauss-Legendre weights 5/9, 8/9, 5/9
-    // Hermite form of the forward dense output (tsit5_dense_hermite): per point {H01, h*H10, h*H11, theta^2 (1-theta)^2}
-    // at the 4 adjoint stage times (rows 0..3, theta of hBst) and at the y-side Gauss nodes (rows 4..6: row 4 + g has the
-    // theta of hBq[2 - g]), and hR4 = h * (theta^4 coefficient of b_j)
+    // Hermite form of the forward dense output: per point {H01, h*H10, h*H11, theta^2 (1-theta)^2} at the 4 adjoint stage
+    // times (rows 0..3, theta of hBst) and at the y-side Gauss nodes (rows 4..6: row 4 + g has the theta of hBq[2 - g]), and
+    // hR4 = h * (theta^4 coefficient of b_j).  The reverse kernel reads the same points with c4's elimination folded in
+    // (OdeRevArgsT::hHf)
     R hHm[7][4];
     R hR4[7];
 };
@@ -102,7 +103,8 @@ template <class R> struct OdeRevArgsT {
     const int32_t* event_of_step; const double* ev_s; const double* ev_c; const double* ev_ps; const double* ev_pc; int32_t nev;   // EV kernels
     R Rpoly[7][4];               // SA_GK: dense-output polynomials b_j(theta) = sum_m Rpoly[j][m] theta^(m+1)
     R hstep;                     // SA_GK: the step size
-    R hC4u[7];                   // tsit5_hermite_c4_du: c4 weights of k1..k5, of du (slot 5, in place of k6) and of k7
+    R hC4u[7];                   // c4 weights of k1..k5, of du (slot 5, in place of k6) and of k7 (tsit5_hermite_c4_du reads 1..4)
+    R hHf[7][4];                 // tsit5_dense_hermite: hHm's points with the c4 elimination folded in (build_hermite_folded)
     P2PComm p2p;                 // fused cross-GPU all-reduce of dp (nranks <= 1: off)
     Tsit5TablesT<R> tb;
 };
@@ -166,31 +168,24 @@ template <int D, class R> __device__ __forceinline__ void tsit5_dense(const R* u
 // The same dense output in Hermite form.  The Tsit5 interpolant is a C1 Hermite quartic: b_j(1) = b_j (row 6 of hA / h),
 // b_j'(0) = delta_j1, b_j'(1) = delta_j7, so with du = u_{n+1} - u_n, k1, k7 = f(u_{n+1}) and c4 = sum_j hR4[j] k_j
 //   y(theta) = u_n + H01 du + h H10 k1 + h H11 k7 + theta^2 (1-theta)^2 c4
-// (H01 = 3t^2 - 2t^3, H10 = t - 2t^2 + t^3, H11 = t^3 - t^2): 4 FMAs per component once c4 and du are formed, against
-// 7 for tsit5_dense.  All weights are <= 1 in magnitude.  u_{n+1} and k7 must be the end point of the SAME step as k1..k6.
-template <int D, class R> __device__ __forceinline__ void tsit5_hermite_c4(const Tsit5TablesT<R>& tb, const R (*k)[D], R* c4) {
-#pragma unroll
-    for (int i = 0; i < D; i++) {
-        R acc = tb.hR4[0] * k[0][i];
-#pragma unroll
-        for (int j = 1; j < 7; j++) acc = fma(tb.hR4[j], k[j][i], acc);
-        c4[i] = acc;
-    }
-}
-// The same c4 without k6.  u_{n+1} = u_n + sum_{j<6} hA[6][j] k_j (b7 = 0), so k6 = (du - sum_{j<5} hA[6][j] k_j) / hA[6][5]
+// (H01 = 3t^2 - 2t^3, H10 = t - 2t^2 + t^3, H11 = t^3 - t^2).  u_{n+1} and k7 must be the end point of the SAME step as k1..k6.
+// k6 need not be formed: u_{n+1} = u_n + sum_{j<6} hA[6][j] k_j (b7 = 0), so k6 = (du - sum_{j<5} hA[6][j] k_j) / hA[6][5]
 // and c4 = sum_{j<5} w_j k_j + w_5 du + hR4[6] k7 with w_j = hR4[j] - hR4[5] b_j / b6 and w_5 = R4[5] / b6 (build_c4_du_weights).
-// A reverse step that has u_{n+1} from the forward pass then rebuilds stages 2..5 only: one RHS call and 5 D stage FMAs
-// fewer.  du carries the rounding of the forward step's sum (about one ulp of u), which |w_5| = 15 and the Hermite
-// weight theta^2 (1-theta)^2 <= 1/16 turn into about one ulp of y.
+// The w_0 k1, w_5 du and w_6 k7 terms then fold into the point weights (build_hermite_folded, a row of OdeRevArgsT::hHf):
+//   y(theta) = u_n + (H01 + G w_5) du + (h H10 + G w_0) k1 + (h H11 + G w_6) k7 + G c4'',   c4'' = sum_{j=1..4} w_j k_j
+// with G = theta^2 (1-theta)^2 <= 1/16: 3 D ops for c4'' (tsit5_hermite_c4_du) and 4 D FMAs per point (tsit5_dense_hermite),
+// against 7 D per point for tsit5_dense.  A reverse step that has u_{n+1} from the forward pass then rebuilds stages 2..5
+// only.  du carries the rounding of the forward step's sum (about one ulp of u), which |H01 + G w_5| <= 1 + 15/16 passes
+// on to y.  The identity is one of the tableau alone, so it holds for the adjoint step's own dense output as well (u_n ->
+// lambda at the step's start, du -> the step's increment, k -> its stages ka').
 template <int D, class R>
-__device__ __forceinline__ void tsit5_hermite_c4_du(const R* w, const R (*k)[D], const R* du, R* c4) {
+__device__ __forceinline__ void tsit5_hermite_c4_du(const R* w, const R (*k)[D], R* c4) {
 #pragma unroll
     for (int i = 0; i < D; i++) {
-        R acc = w[0] * k[0][i];
+        R acc = w[1] * k[1][i];
 #pragma unroll
-        for (int j = 1; j < 5; j++) acc = fma(w[j], k[j][i], acc);
-        acc = fma(w[5], du[i], acc);
-        c4[i] = fma(w[6], k[6][i], acc);
+        for (int j = 2; j < 5; j++) acc = fma(w[j], k[j][i], acc);
+        c4[i] = acc;
     }
 }
 template <int D, class R>
@@ -677,16 +672,16 @@ __global__ void __maxnreg__(B200_REV_MAXREG) tsit5_reverse_kernel(const __grid_c
             if (grp < 0) continue;             // resting warp of the rotating row: barriers only
 
             // ---- forward stage recompute on [t_n, t_{n+1}]: the dense-output data of this step ----
-            // k6 only where something needs more than c4: GaussKronrod's general-theta dense output and the event kernels'
-            // left limit (stage 6 re-derived); elsewhere c4 comes from du in its place (tsit5_hermite_c4_du)
-            constexpr bool K6 = EV || SA == SA_GK;
+            // k6 only where something needs more than the Hermite data: GaussKronrod's general-theta dense output and the
+            // event kernels' left limit (stage 6 re-derived); the Hermite points take du in its place (tsit5_hermite_c4_du)
+            constexpr bool K6 = SA == SA_GK;
             R tmp[D];
             Fam::f(ulo, p, kf[0]);
             tsit5_stage<D, 1>(tb, ulo, kf, tmp); Fam::f(tmp, p, kf[1]);
             tsit5_stage<D, 2>(tb, ulo, kf, tmp); Fam::f(tmp, p, kf[2]);
             tsit5_stage<D, 3>(tb, ulo, kf, tmp); Fam::f(tmp, p, kf[3]);
             tsit5_stage<D, 4>(tb, ulo, kf, tmp); Fam::f(tmp, p, kf[4]);
-            if (K6) { tsit5_stage<D, 5>(tb, ulo, kf, tmp); Fam::f(tmp, p, kf[5]); }
+            if (K6 || (EV && need_left)) { tsit5_stage<D, 5>(tb, ulo, kf, tmp); Fam::f(tmp, p, kf[5]); }
 
             if (EV && need_left) {
                 // the step above ended with an event at t_{n+1}: the first adjoint stage sees the LEFT limit there -- the end
@@ -698,12 +693,12 @@ __global__ void __maxnreg__(B200_REV_MAXREG) tsit5_reverse_kernel(const __grid_c
                 need_left = false;
             }
             // Hermite data of the forward dense output: uhi / kf[6] are this step's end point (the checkpoint u_{n+1} and its
-            // FSAL derivative, or the re-derived left limit at an event); kf[1..5] are dead from here on (except for GK)
+            // FSAL derivative, or the re-derived left limit at an event, so du is this step's own increment); kf[1..5] are
+            // dead from here on (except for GK)
             R du[D], c4[D];
 #pragma unroll
             for (int j = 0; j < D; j++) du[j] = uhi[j] - ulo[j];
-            if (K6) tsit5_hermite_c4<D>(tb, kf, c4);
-            else tsit5_hermite_c4_du<D>(a.hC4u, kf, du, c4);
+            tsit5_hermite_c4_du<D>(a.hC4u, kf, c4);
 #ifdef REV_MIDSYNC
             __syncthreads();
 #endif
@@ -721,10 +716,10 @@ __global__ void __maxnreg__(B200_REV_MAXREG) tsit5_reverse_kernel(const __grid_c
             Fam::vjp_u(y, p, ls, ka[S_]); add_continuous<D, CONT>(a, y, ka[S_]);                 \
             if (SA == SA_INTERP && S_ < 6) { Fam::vjp_p(y, p, ls, dg);                     \
                 _Pragma("unroll") for (int q = 0; q < P; q++) mu[q] = fma(tb.hA[6][S_ < 6 ? S_ : 0], dg[q], mu[q]); }
-            B200_ADJ_STAGE(1, tsit5_dense_hermite<D>(ulo, du, kf[0], kf[6], c4, tb.hHm[0], y))
-            B200_ADJ_STAGE(2, tsit5_dense_hermite<D>(ulo, du, kf[0], kf[6], c4, tb.hHm[1], y))
-            B200_ADJ_STAGE(3, tsit5_dense_hermite<D>(ulo, du, kf[0], kf[6], c4, tb.hHm[2], y))
-            B200_ADJ_STAGE(4, tsit5_dense_hermite<D>(ulo, du, kf[0], kf[6], c4, tb.hHm[3], y))
+            B200_ADJ_STAGE(1, tsit5_dense_hermite<D>(ulo, du, kf[0], kf[6], c4, a.hHf[0], y))
+            B200_ADJ_STAGE(2, tsit5_dense_hermite<D>(ulo, du, kf[0], kf[6], c4, a.hHf[1], y))
+            B200_ADJ_STAGE(3, tsit5_dense_hermite<D>(ulo, du, kf[0], kf[6], c4, a.hHf[2], y))
+            B200_ADJ_STAGE(4, tsit5_dense_hermite<D>(ulo, du, kf[0], kf[6], c4, a.hHf[3], y))
             B200_ADJ_STAGE(5, _Pragma("unroll") for (int j = 0; j < D; j++) y[j] = ulo[j])
             B200_ADJ_STAGE(6, _Pragma("unroll") for (int j = 0; j < D; j++) y[j] = ulo[j])
 #undef B200_ADJ_STAGE
@@ -771,12 +766,17 @@ __global__ void __maxnreg__(B200_REV_MAXREG) tsit5_reverse_kernel(const __grid_c
             }
             if (SA == SA_GAUSS) {
                 // 3-point Gauss-Legendre over this step, pre-jump lambda from the adjoint step's own dense output,
-                // y from the forward dense output: dp += (h/2) w_q (df/dp)'(y_q) lam_q  (gauss_adjoint.jl:745-759)
-                R lq[D];
+                // y from the forward dense output: dp += (h/2) w_q (df/dp)'(y_q) lam_q  (gauss_adjoint.jl:745-759).
+                // Both in Hermite form: lambda at theta_g of the adjoint step (start lam, increment ls - lam, end-point
+                // derivatives ka[0], ka[6]) is the point of the y-side row with theta 1 - theta_g = theta_{2-g}, row 6 - g
+                R dl[D], cl[D], lq[D];
+#pragma unroll
+                for (int j = 0; j < D; j++) dl[j] = ls[j] - lam[j];
+                tsit5_hermite_c4_du<D>(a.hC4u, ka, cl);
 #pragma unroll
                 for (int g = 0; g < 3; g++) {
-                    tsit5_dense<D>(lam, ka, tb.hBq[g], lq);
-                    tsit5_dense_hermite<D>(ulo, du, kf[0], kf[6], c4, tb.hHm[4 + g], y);
+                    tsit5_dense_hermite<D>(lam, dl, ka[0], ka[6], cl, a.hHf[6 - g], lq);
+                    tsit5_dense_hermite<D>(ulo, du, kf[0], kf[6], c4, a.hHf[4 + g], y);
                     Fam::vjp_p(y, p, lq, dg);
 #pragma unroll
                     for (int q = 0; q < P; q++) mu[q] = fma(tb.hGW[g], dg[q], mu[q]);
