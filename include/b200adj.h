@@ -46,7 +46,9 @@ enum {
  * scimlsensitivity_jl_b200.family_plugin builds it).  Registering it yields a family id for cfg.rhs_family.  F64; fixed-step
  * and adaptive Tsit5 with all sensealgs and events; Rosenbrock23 when the struct also supplies jac / djac / dvjp_p.  A
  * diagonal-noise SDE family (B200ADJ_FAMILY_SDE: drift f, diffusion g and their VJPs) runs on EM / EulerHeun with
- * BacksolveAdjoint / InterpolatingAdjoint, and on no ODE stepper. */
+ * BacksolveAdjoint / InterpolatingAdjoint, and on no ODE stepper.  So does a general-noise SDE family
+ * (B200ADJ_FAMILY_SDE_GENERAL: a D x M diffusion G with 1 <= M <= 4 -- scalar noise M = 1, non-diagonal, non-square, or diagonal
+ * noise that mixes), except EM with BacksolveAdjoint. */
 #define B200ADJ_FAM_USER_BASE 100
 int32_t b200adj_register_family(const char* plugin_path, int32_t* family_id);
 int32_t b200adj_family_info(int32_t family_id, int32_t* d, int32_t* P, const char** name);
@@ -220,10 +222,21 @@ int32_t b200adj_event_times(void* handle, int32_t* counts, double* times);
 /* Number of conditions compiled into a family (its plug-in was built with B200ADJ_FAMILY_HAS_EVENTS, csrc/family_plugin.inc):
  * the `len` of VectorContinuousCallback(condition, affect!, len).  0 for every built-in family and for plug-ins without events. */
 int32_t b200adj_family_conditions(int32_t family, int32_t* nc);
-/* Number of Wiener processes of a family (the m of the SDE steppers EM / EulerHeun; diagonal noise, so m = d): 2 for the
- * built-in SDE_LV / SDE_LINEAR, M for a plug-in built with B200ADJ_FAMILY_SDE (csrc/family_plugin.inc), 0 for every ODE
- * family.  B200ADJ_ERR_INVALID for an unknown family id. */
+/* Number of Wiener processes of a family (the m of the SDE steppers EM / EulerHeun; m = d for diagonal noise): 2 for the
+ * built-in SDE_LV / SDE_LINEAR, M for a plug-in built with B200ADJ_FAMILY_SDE or B200ADJ_FAMILY_SDE_GENERAL
+ * (csrc/family_plugin.inc), 0 for every ODE family.  B200ADJ_ERR_INVALID for an unknown family id. */
 int32_t b200adj_family_noise(int32_t family, int32_t* m);
+/* The shape of a family's noise term (the reference's noise_rate_prototype):
+ *   B200ADJ_NOISE_NONE      an ODE family
+ *   B200ADJ_NOISE_DIAGONAL  du = f dt + g .* dW, m = d, g_i a function of u_i and p (the built-in SDE_LV / SDE_LINEAR and the
+ *                           plug-ins built with B200ADJ_FAMILY_SDE; noisemixing = false)
+ *   B200ADJ_NOISE_GENERAL   du = f dt + G dW with G of size d x m (plug-ins built with B200ADJ_FAMILY_SDE_GENERAL); the
+ *                           diffusion VJP is the full one of noisemixing = true.  EM + BacksolveAdjoint is UNSUPPORTED: the
+ *                           reference's Ito-transformed drift (src/sde_tools.jl:29-66) is not the Ito correction of a noise
+ *                           that mixes.
+ * B200ADJ_ERR_INVALID for an unknown family id. */
+enum { B200ADJ_NOISE_NONE = 0, B200ADJ_NOISE_DIAGONAL = 1, B200ADJ_NOISE_GENERAL = 2 };
+int32_t b200adj_family_noise_kind(int32_t family, int32_t* kind);
 /* VectorContinuousCallback of the reference (the callback type of test/Callbacks2/vector_continuous_callbacks.jl; reverse-pass
  * treatment of src/callback_tracking.jl:232-480) with the condition(out, u, t, integrator) and affect!(integrator, ev) compiled
  * into the family struct, save_positions = (false, false).  A mode of the continuous callback above: each member finds its own

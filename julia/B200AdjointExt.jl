@@ -128,6 +128,21 @@ last_error(h) = unsafe_string(ccall((:b200adj_last_error, libb200adj), Cstring, 
 # UNSUPPORTED -> a dedicated exception the entry points turn into delegation; everything else is an error
 check(h, rc) = rc == 0 ? nothing : rc == ERR_UNSUPPORTED ? throw(B200Unsupported(last_error(h))) : error("b200adj error $rc: " * last_error(h))
 
+const NOISE_NONE, NOISE_DIAGONAL, NOISE_GENERAL = Int32(0), Int32(1), Int32(2)
+"""
+    family_noise_kind(family) -> NOISE_NONE, NOISE_DIAGONAL or NOISE_GENERAL
+
+The shape of a family's noise term (`b200adj_family_noise_kind`).  A general-noise SDE plug-in (`B200ADJ_FAMILY_SDE_GENERAL`,
+G of size d x m) serves an `SDEProblem` with `noise_rate_prototype` of that size (scalar, non-diagonal or mixing noise);
+EM + BacksolveAdjoint on it is UNSUPPORTED and so delegated to the wrapped sensealg.
+"""
+function family_noise_kind(family::Integer)
+    k = Ref{Int32}(0)
+    rc = ccall((:b200adj_family_noise_kind, libb200adj), Int32, (Int32, Ref{Int32}), Int32(family), k)
+    rc == 0 || error("b200adj_family_noise_kind: unknown family id $family")
+    return k[]
+end
+
 mutable struct Handle
     ptr::Ptr{Cvoid}
     function Handle(cfg::B200Cfg)

@@ -19,9 +19,10 @@ ST = {"tsit5_fixed": 0, "rosenbrock23": 1, "em": 2, "euler_heun": 3, "tsit5_adap
 DTYPE = {"f64": 0, "f32": 1, "bf16_f32acc": 2}
 COST = {"explicit": 0, "affine": 1}
 FLAG_NO_START, FLAG_NO_CHECKPOINTING, FLAG_CKPT_EVERY_STEP, FLAG_STORED_NOISE, FLAG_TRACE, FLAG_NO_ROTATE, FLAG_DENSE_FORWARD, FLAG_NCCL_ALLREDUCE = 1, 2, 4, 8, 16, 32, 64, 128
+NOISE_NONE, NOISE_DIAGONAL, NOISE_GENERAL = 0, 1, 2
 ERR = {0: "OK", -1: "INVALID", -2: "UNSUPPORTED", -3: "NO_DEVICE", -4: "CUDA", -5: "STATE", -6: "OOM"}
 
-EXPORTS = ["b200adj_create", "b200adj_forward", "b200adj_reverse", "b200adj_set_reverse_options", "b200adj_set_tolerances", "b200adj_set_continuous_cost", "b200adj_set_cost_family", "b200adj_register_family", "b200adj_family_info", "b200adj_set_events", "b200adj_set_event_param_shift", "b200adj_set_continuous_callback", "b200adj_set_continuous_callback_params", "b200adj_event_times", "b200adj_family_conditions", "b200adj_family_noise", "b200adj_set_family_events", "b200adj_event_flags", "b200adj_get_noise", "b200adj_set_stream",
+EXPORTS = ["b200adj_create", "b200adj_forward", "b200adj_reverse", "b200adj_set_reverse_options", "b200adj_set_tolerances", "b200adj_set_continuous_cost", "b200adj_set_cost_family", "b200adj_register_family", "b200adj_family_info", "b200adj_set_events", "b200adj_set_event_param_shift", "b200adj_set_continuous_callback", "b200adj_set_continuous_callback_params", "b200adj_event_times", "b200adj_family_conditions", "b200adj_family_noise", "b200adj_family_noise_kind", "b200adj_set_family_events", "b200adj_event_flags", "b200adj_get_noise", "b200adj_set_stream",
            "b200adj_synchronize", "b200adj_launch_count", "b200adj_get_step_counts", "b200adj_get_block_trace", "b200adj_destroy",
            "b200adj_last_error", "b200adj_version", "b200adj_sizeof_cfg",
            "b200adj_comm_unique_id", "b200adj_comm_init", "b200adj_comm_init_all", "b200adj_comm_allreduce", "b200adj_comm_size", "b200adj_comm_is_fused"]
@@ -154,6 +155,8 @@ def load():
         lib.b200adj_family_conditions.restype = C.c_int32
         lib.b200adj_family_noise.argtypes = [C.c_int32, C.POINTER(C.c_int32)]
         lib.b200adj_family_noise.restype = C.c_int32
+        lib.b200adj_family_noise_kind.argtypes = [C.c_int32, C.POINTER(C.c_int32)]
+        lib.b200adj_family_noise_kind.restype = C.c_int32
         lib.b200adj_set_family_events.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32]
         lib.b200adj_set_family_events.restype = C.c_int32
         lib.b200adj_event_flags.argtypes = [C.c_void_p, C.c_void_p]
@@ -215,12 +218,22 @@ def family_conditions(family_id):
 
 
 def family_noise(family_id):
-    """Number of Wiener processes of a family: m = d for a diagonal-noise SDE family, 0 for an ODE family."""
+    """Number of Wiener processes of a family: m = d for a diagonal-noise SDE family, the M of a general-noise one, 0 for an
+    ODE family."""
     m = C.c_int32()
     rc = load().b200adj_family_noise(int(family_id), C.byref(m))
     if rc != 0:
         raise B200AdjError(rc, f"unknown family id {family_id}")
     return m.value
+
+
+def family_noise_kind(family_id):
+    """Shape of a family's noise term: NOISE_NONE (ODE family), NOISE_DIAGONAL (g .* dW) or NOISE_GENERAL (G dW, G of size d x m)."""
+    k = C.c_int32()
+    rc = load().b200adj_family_noise_kind(int(family_id), C.byref(k))
+    if rc != 0:
+        raise B200AdjError(rc, f"unknown family id {family_id}")
+    return k.value
 
 
 def comm_unique_id():

@@ -11,11 +11,11 @@ import numpy as np
 
 from . import distributed
 from .engine import DeviceEnsemble, _is_torch
-from .problems import (EM, AffineCost, ContinuousCallback, VectorContinuousCallback, PresetTimeCallback, EnsembleB200, EnsembleProblem, EnsembleSolution, EulerHeun, FAMILIES, ODEProblem,
+from .problems import (EM, AffineCost, ContinuousCallback, VectorContinuousCallback, PresetTimeCallback, EnsembleB200, EnsembleProblem, EnsembleSolution, EulerHeun, FAMILIES, GENERAL_NOISE_FAMILIES, ODEProblem,
                        Rosenbrock23, SDEProblem, Tsit5, saveat_to_times)
 from .sensitivity_algorithms import (B200Adjoint, BacksolveAdjoint, GaussAdjoint, GaussKronrodAdjoint, InterpolatingAdjoint,
                                      QuadratureAdjoint, sensealg_name)
-from .sensitivity_interface import _check_noise_mixing, _check_params, adjoint_sensitivities
+from .sensitivity_interface import _check_general_noise, _check_noise_mixing, _check_params, adjoint_sensitivities
 
 
 class NoTangent:
@@ -56,6 +56,17 @@ def _materialise(eprob, trajectories):
         u0s = np.repeat(np.asarray(prob.u0, dtype=np.float64).reshape(-1, 1), trajectories, axis=1)
         ps = None
     return u0s, ps
+
+
+def _check_noise_rate_prototype(prob, d, m):
+    """SDEProblem(...; noise_rate_prototype): only a general-noise family takes one, of its own shape (d, m)"""
+    proto = getattr(prob, "noise_rate_prototype", None)
+    if proto is None:
+        return
+    if prob.f not in GENERAL_NOISE_FAMILIES:
+        raise ValueError(f"noise_rate_prototype: {prob.f!r} is not a general-noise SDE family (build it with noise=\"general\")")
+    if tuple(np.shape(proto)) != (d, m):
+        raise ValueError(f"noise_rate_prototype has shape {tuple(np.shape(proto))}; the family {prob.f!r} has a ({d}, {m}) diffusion")
 
 
 def _step_size(alg, kwargs):
@@ -114,6 +125,8 @@ def solve(eprob, alg, ensemblealg=None, *, trajectories=None, saveat=None, sense
         raise KeyError(f"unknown RHS family {prob.f!r}; known: {sorted(FAMILIES)}")
     d, P, m = FAMILIES[prob.f]
     _check_noise_mixing(prob.f, sensealg)
+    _check_general_noise(prob.f, alg.code, sensealg)
+    _check_noise_rate_prototype(prob, d, m)
     if u0 is None or p is None:
         if trajectories is None:
             trajectories = eprob.u0s.shape[1] if eprob.u0s is not None else 1

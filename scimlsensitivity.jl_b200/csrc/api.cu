@@ -40,7 +40,7 @@ FamilyVTable builtin_family(const char* name) {
 template <template <bool> class F>
 FamilyVTable builtin_sde_family(const char* name) {
     FamilyVTable v = {B200ADJ_PLUGIN_ABI, F<false>::D, F<false>::P, name};
-    v.m = F<false>::M; v.sde_fwd = &launch_sde_fwd<F>; v.sde_rev = &launch_sde_rev<F>;
+    v.m = F<false>::M; v.noise = B200ADJ_NOISE_DIAGONAL; v.sde_fwd = &launch_sde_fwd<F>; v.sde_rev = &launch_sde_rev<F>;
     return v;
 }
 constexpr int BUILTIN_FAMILIES = B200ADJ_FAM_RELAX + 1;
@@ -91,6 +91,12 @@ int32_t check_support(const b200adj_cfg& c, Path path, int ckpt_every, int32_t s
     if (rules & SR_SENSEALG) {
         if (path == Path::SDE && sensealg != B200ADJ_SA_BACKSOLVE && sensealg != B200ADJ_SA_INTERPOLATING)
             return refuse("SDE: BacksolveAdjoint / InterpolatingAdjoint are built");
+        // BacksolveAdjoint on an Ito solver integrates the reference's transformed drift f - J_{vec G}' vec G, which is the
+        // Ito correction only for noise that does not mix (DESIGN.md section 4.3)
+        if (path == Path::SDE && sensealg == B200ADJ_SA_BACKSOLVE && c.stepper == B200ADJ_ST_EM) {
+            const FamilyVTable* vt = family_lookup(c.rhs_family);
+            if (vt && vt->noise == B200ADJ_NOISE_GENERAL) return refuse("general-noise SDE family: EM + BacksolveAdjoint is not built (use EulerHeun or InterpolatingAdjoint)");
+        }
         if (sensealg < 0 || sensealg > 4) { err = "bad sensealg"; return B200ADJ_ERR_INVALID; }
         if (sensealg == B200ADJ_SA_GAUSSKRONROD && c.dtype != B200ADJ_F64) return refuse("GaussKronrodAdjoint: F64, named ODE families");
     }
@@ -601,8 +607,11 @@ int32_t b200adj_register_family(const char* plugin_path, int32_t* family_id) {
     // a refused plug-in is unloaded again, so that a rebuilt file of the same name is really loaded next time
     if (!vt || vt->abi != B200ADJ_PLUGIN_ABI) { dlclose(lib); g_create_error = "register_family: plug-in built against other headers (ABI tag mismatch): rebuild it"; return B200ADJ_ERR_INVALID; }
     if (vt->d < 1 || vt->d > 4 || vt->P < 1 || vt->P > 8) { dlclose(lib); g_create_error = "register_family: 1 <= D <= 4 and 1 <= P <= 8"; return B200ADJ_ERR_UNSUPPORTED; }
-    if (vt->m != 0 && (vt->m != vt->d || !vt->sde_fwd || !vt->sde_rev)) {
-        dlclose(lib); g_create_error = "register_family: an SDE plug-in has diagonal noise (M == D) and the EM / EulerHeun launchers"; return B200ADJ_ERR_UNSUPPORTED; }
+    if (vt->m != 0 && (!vt->sde_fwd || !vt->sde_rev ||
+                       !(vt->noise == B200ADJ_NOISE_DIAGONAL ? vt->m == vt->d : vt->noise == B200ADJ_NOISE_GENERAL && vt->m >= 1 && vt->m <= 4))) {
+        dlclose(lib); g_create_error = "register_family: an SDE plug-in has the EM / EulerHeun launchers and diagonal noise (M == D) or general noise (1 <= M <= 4)";
+        return B200ADJ_ERR_UNSUPPORTED; }
+    if (vt->m == 0 && vt->noise != B200ADJ_NOISE_NONE) { dlclose(lib); g_create_error = "register_family: an ODE plug-in has no noise"; return B200ADJ_ERR_INVALID; }
     auto& r = family_registry();
     for (size_t k = 0; k < r.size(); k++) if (r[k] == vt) { *family_id = B200ADJ_FAM_USER_BASE_ID + (int)k; return B200ADJ_OK; }
     r.push_back(vt);
@@ -788,6 +797,14 @@ int32_t b200adj_family_noise(int32_t family, int32_t* m) {
     if (const FamilyVTable* vt = family_lookup(family)) { *m = vt->m; return B200ADJ_OK; }
     for (const FamDims& f : OWN_DISPATCH_FAMILIES)
         if (f.id == family) { *m = f.m; return B200ADJ_OK; }
+    return B200ADJ_ERR_INVALID;
+}
+
+int32_t b200adj_family_noise_kind(int32_t family, int32_t* kind) {
+    if (!kind) return B200ADJ_ERR_INVALID;
+    if (const FamilyVTable* vt = family_lookup(family)) { *kind = vt->noise; return B200ADJ_OK; }
+    for (const FamDims& f : OWN_DISPATCH_FAMILIES)
+        if (f.id == family) { *kind = B200ADJ_NOISE_NONE; return B200ADJ_OK; }
     return B200ADJ_ERR_INVALID;
 }
 

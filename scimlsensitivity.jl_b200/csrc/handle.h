@@ -150,7 +150,9 @@ template <class T, class S> inline void cast_tables(const S& src, T* dst) {
 // ---- family registry (SURVEY.md 8f rank 4; the seam user-supplied ODEFunction(f; vjp, vjp_p, jac, paramjac) occupies in the
 // reference, src/derivative_wrappers.jl:284-359, test/Core3/user_vjp.jl:14-38).  A family PLUG-IN is a shared library built from
 // a user header that defines one struct with the shape of families.cuh (D, P, f, vjp_u, vjp_p [, jac, djac, dvjp_p]), or for a
-// diagonal-noise SDE one `template <bool ITO> struct` with the shape of SdeLotkaVolterra (D, P, M = D, f, g and their VJPs);
+// diagonal-noise SDE one `template <bool ITO> struct` with the shape of SdeLotkaVolterra (D, P, M = D, f, g and their VJPs),
+// or for a general-noise SDE one plain struct (D, P, M, f and its VJPs, and the contractions g_apply / gvjp_u_apply /
+// gvjp_p_apply of its D x M diffusion with the increments; sde_em.cuh);
 // the plug-in instantiates the same kernel templates for it and exports this table of launchers (family_plugin.inc).
 // b200adj_register_family(path) loads it and hands out a family id >= B200ADJ_FAM_USER_BASE.  The built-in families fill
 // the same table (api.cu, builtin_families), so every family but MLP dispatches through one lookup. ----
@@ -168,10 +170,11 @@ struct FamilyVTable {
     int (*rev_f32)(Handle*, const OdeRevArgsT<float>&);
     int32_t nc;                   // conditions of the family's own state-dependent event (B200ADJ_FAMILY_HAS_EVENTS); 0: none
     int32_t m;                    // Wiener processes of an SDE family (diagonal noise: m = d); 0: an ODE family
+    int32_t noise;                // B200ADJ_NOISE_*: NONE for an ODE family, DIAGONAL or GENERAL for an SDE family
     int (*sde_fwd)(Handle*, const SdeFwdArgs&);      // EM / EulerHeun (SDE families only; null for an ODE family)
     int (*sde_rev)(Handle*, const SdeRevArgs&);
 };
-constexpr uint32_t B200ADJ_PLUGIN_ABI = 0x00020000u ^ (uint32_t)sizeof(Handle) ^ ((uint32_t)sizeof(OdeRevArgs) << 8) ^
+constexpr uint32_t B200ADJ_PLUGIN_ABI = 0x00030000u ^ (uint32_t)sizeof(Handle) ^ ((uint32_t)sizeof(OdeRevArgs) << 8) ^
                                         ((uint32_t)sizeof(T5aArgs) << 16) ^ ((uint32_t)sizeof(FamilyVTable) << 24) ^
                                         ((uint32_t)sizeof(SdeFwdArgs) << 4) ^ ((uint32_t)sizeof(SdeRevArgs) << 12);
 constexpr int B200ADJ_FAM_USER_BASE_ID = 100;

@@ -1,4 +1,5 @@
-// sde_em.cuh -- diagonal-noise SDE ensemble kernels: forward EM / EulerHeun and the BacksolveAdjoint reverse pass.
+// sde_em.cuh -- SDE ensemble kernels: forward EM / EulerHeun and the BacksolveAdjoint / InterpolatingAdjoint reverse pass,
+// for diagonal noise (g .* dW) and for general noise (G dW, G of size D x M).
 // One member per thread, SoA [step][dim][member].  Wiener increments come from a Philox4x32-10 counter keyed by
 // (seed, global member index, step) so the reverse pass REGENERATES them instead of reading a stored noise grid
 // (the reference stores sol.W and integrates against reverse(W), src/backsolve_adjoint.jl:395-411); a stored-noise
@@ -6,7 +7,7 @@
 //
 // Reference functions replaced:  SDEAdjointProblem src/backsolve_adjoint.jl:274-419 (state z=[lam; mu; y], drift
 // functor on f or on the Ito-transformed drift :327-345, diffusion functor noiseterm=true :347-357), sense functor
-// arithmetic :32-61, diagonal-noise layout split_states :92-100, jacNoise! src/derivative_wrappers.jl:1165-1211,
+// arithmetic :32-61, noise layouts split_states :92-117, jacNoise! src/derivative_wrappers.jl:1165-1258,
 // StochasticTransformedFunction src/sde_tools.jl:29-66, checkpoint reset :523-546, ReverseLossCallback
 // src/adjoint_common.jl:754-821; upstream EM / EulerHeun steps (SURVEY.md App. B).
 #pragma once
@@ -81,11 +82,49 @@ __global__ void sde_noise_kernel(SdeNoiseArgs a) {
     }
 }
 
+// The two noise shapes of an SDE family.  Diagonal (SdeLotkaVolterra): g(u, p, g) gives the diffusion of each component,
+// one Wiener process per state (M == D), and the noise enters as g .* w.  General (a struct with g_apply): G(u, p) is D x M
+// and the family supplies only its contractions with the increments w[M] -- the noise enters linearly, so the kernels never
+// form the matrix the reference builds and multiplies by dW (src/derivative_wrappers.jl:1197-1258):
+//   g_apply(u, p, w, out)            out = G w
+//   gvjp_u_apply(u, p, l, w, dl)     dl = sum_j w_j (dG[:, j]/du)' l
+//   gvjp_p_apply(u, p, l, w, dg)     dg = sum_j w_j (dG[:, j]/dp)' l        (the same name and meaning in both shapes)
+// Each helper below has one form per shape; the diagonal forms are the expressions the kernels had before the general
+// shape existed.
+template <class Fam, class = void> struct SdeGeneralNoise { static constexpr bool value = false; };
+template <class Fam> struct SdeGeneralNoise<Fam, decltype(void(&Fam::template g_apply<double>))> { static constexpr bool value = true; };
+
+// the diffusion at (u, p) in the family's form: g (diagonal) or G w (general)
+template <class Fam>
+__device__ __forceinline__ void sde_diffusion(const double* u, const double* p, const double* w, double* g) {
+    if constexpr (SdeGeneralNoise<Fam>::value) Fam::g_apply(u, p, w, g);
+    else Fam::g(u, p, g);
+}
+// its noise term in component j: g_j w_j or (G w)_j
+template <class Fam>
+__device__ __forceinline__ double sde_noise(const double* g, const double* w, int j) {
+    if constexpr (SdeGeneralNoise<Fam>::value) return g[j];
+    else return g[j] * w[j];
+}
+// EulerHeun's averaged noise term from the diffusions at u and at the predictor
+template <class Fam>
+__device__ __forceinline__ double sde_noise_avg(const double* g, const double* gb, const double* w, int j) {
+    if constexpr (SdeGeneralNoise<Fam>::value) return 0.5 * (g[j] + gb[j]);
+    else return 0.5 * (g[j] + gb[j]) * w[j];
+}
+// the u-part of the diffusion VJP in the family's form: l .* dg/du (diagonal) or sum_j w_j (dG[:, j]/du)' l (general);
+// sde_noise turns either into the reverse diffusion increment
+template <class Fam>
+__device__ __forceinline__ void sde_diffusion_vjp_u(const double* u, const double* p, const double* l, const double* w, double* dl) {
+    if constexpr (SdeGeneralNoise<Fam>::value) Fam::gvjp_u_apply(u, p, l, w, dl);
+    else Fam::gvjp_u(u, p, l, dl);
+}
+
 template <class Fam, bool EULER_HEUN, bool SHARED_P>
 __global__ void __launch_bounds__(512) sde_forward_kernel(SdeFwdArgs a) {
     const int BLOCK = (int)blockDim.x;
     constexpr int D = Fam::D, P = Fam::P, M = Fam::M;
-    static_assert(M == D, "diagonal noise: one Wiener process per state");
+    static_assert(SdeGeneralNoise<Fam>::value || M == D, "diagonal noise: one Wiener process per state");
     const int64_t gi = (int64_t)blockIdx.x * BLOCK + threadIdx.x;
     const bool active = gi < a.N;
     const int64_t i = active ? gi : a.N - 1;
@@ -104,17 +143,17 @@ __global__ void __launch_bounds__(512) sde_forward_kernel(SdeFwdArgs a) {
         if (a.noise_in) load_state<M>(a.noise_in + (int64_t)n * M * N, N, i, dW);
         else wiener_increment<M>(a.seed, (uint64_t)(a.traj_offset + i), (uint32_t)n, sq, dW);
         if (a.noise_out && active) store_state<M>(a.noise_out + (int64_t)n * M * N, N, i, dW);
-        Fam::f(u, p, f); Fam::g(u, p, g);
+        Fam::f(u, p, f); sde_diffusion<Fam>(u, p, dW, g);
         if (!EULER_HEUN) {
 #pragma unroll
-            for (int j = 0; j < D; j++) u[j] = u[j] + h * f[j] + g[j] * dW[j];
+            for (int j = 0; j < D; j++) u[j] = u[j] + h * f[j] + sde_noise<Fam>(g, dW, j);
         } else {
             double ub[D], fb[D], gb[D];
 #pragma unroll
-            for (int j = 0; j < D; j++) ub[j] = u[j] + h * f[j] + g[j] * dW[j];
-            Fam::f(ub, p, fb); Fam::g(ub, p, gb);
+            for (int j = 0; j < D; j++) ub[j] = u[j] + h * f[j] + sde_noise<Fam>(g, dW, j);
+            Fam::f(ub, p, fb); sde_diffusion<Fam>(ub, p, dW, gb);
 #pragma unroll
-            for (int j = 0; j < D; j++) u[j] = u[j] + 0.5 * h * (f[j] + fb[j]) + 0.5 * (g[j] + gb[j]) * dW[j];
+            for (int j = 0; j < D; j++) u[j] = u[j] + 0.5 * h * (f[j] + fb[j]) + sde_noise_avg<Fam>(g, gb, dW, j);
         }
         if (active) {
             store_state<D>(a.ckpt + (int64_t)(n + 1) * stride, N, i, u);
@@ -135,9 +174,9 @@ __device__ __forceinline__ void sde_adj_terms(const double* lam, const double* y
                                               double* al, double* am, double* ay, double* bl, double* bm, double* by) {
     double g[D], gl[D];
     Fam::vjp_u(y, p, lam, al); Fam::vjp_p(y, p, lam, am); Fam::f(y, p, ay);
-    Fam::g(y, p, g); Fam::gvjp_u(y, p, lam, gl); Fam::gvjp_p_apply(y, p, lam, w, bm);
+    sde_diffusion<Fam>(y, p, w, g); sde_diffusion_vjp_u<Fam>(y, p, lam, w, gl); Fam::gvjp_p_apply(y, p, lam, w, bm);
 #pragma unroll
-    for (int j = 0; j < D; j++) { al[j] = -al[j]; bl[j] = -gl[j] * w[j]; by[j] = g[j] * w[j]; }
+    for (int j = 0; j < D; j++) { al[j] = -al[j]; bl[j] = -sde_noise<Fam>(gl, w, j); by[j] = sde_noise<Fam>(g, w, j); }
 #pragma unroll
     for (int q = 0; q < P; q++) { am[q] = -am[q]; bm[q] = -bm[q]; }
 }

@@ -20,6 +20,8 @@ FAMILIES = {
 }
 # conditions compiled into a registered plug-in family (VectorContinuousCallback); families not listed have none
 FAMILY_CONDITIONS = {}
+# registered SDE plug-in families with general noise (G of size d x m); every other SDE family has diagonal noise
+GENERAL_NOISE_FAMILIES = set()
 
 
 class AdjointSensitivityParameterCompatibilityError(TypeError):
@@ -45,7 +47,11 @@ class ODEProblem:
 
 @dataclass
 class SDEProblem:
-    f: str                       # named drift+diffusion family (diagonal noise)
+    """SDEProblem(f, u0, tspan, p; noise_rate_prototype).  `f` names a drift + diffusion family: diagonal noise g .* dW, or
+    general noise G dW with G of size (d, m) (a plug-in built with noise="general").  noise_rate_prototype, as in the
+    reference, marks non-diagonal noise: for a general-noise family it may be given (any array of shape (d, m) of the
+    family; its values are not used), for a diagonal one it must be None.  A mismatch raises ValueError in solve()."""
+    f: str                       # named drift+diffusion family
     u0: Any
     tspan: tuple
     p: Any = None
@@ -53,6 +59,7 @@ class SDEProblem:
     seed: int = 0
     noise: Any = None            # explicit Wiener increments dW[S][m][N] (NoiseGrid-like)
     kwargs: dict = field(default_factory=dict)
+    noise_rate_prototype: Any = None
     is_sde = True
 
 

@@ -9,7 +9,8 @@ src/sensitivity_interface.jl:503-507).  For an ensemble `du0` is [d, N]; with pe
 import numpy as np
 
 from . import _lib
-from .problems import FAMILIES, AdjointSensitivityParameterCompatibilityError, AffineCost, ParamAffine, QuadraticRunningCost
+from .problems import (FAMILIES, GENERAL_NOISE_FAMILIES, AdjointSensitivityParameterCompatibilityError, AffineCost, ParamAffine,
+                       QuadraticRunningCost)
 from .sensitivity_algorithms import (B200Adjoint, BacksolveAdjoint, GaussAdjoint, GaussKronrodAdjoint, InterpolatingAdjoint,
                                      QuadratureAdjoint, isnoisemixing, sensealg_name)
 
@@ -17,13 +18,24 @@ FAM_USER_BASE = 100      # B200ADJ_FAM_USER_BASE: ids of registered plug-in fami
 
 
 def _check_noise_mixing(family, sensealg):
-    """A plug-in SDE family's kernels take g_i to depend on u_i and p only (csrc/family_plugin.inc): the noisemixing = true
-    diffusion VJP of the reference (src/derivative_wrappers.jl:1165-1211) is not built for it."""
-    if sensealg is None or not isnoisemixing(sensealg):
+    """A diagonal-noise plug-in SDE family's kernels take g_i to depend on u_i and p only (csrc/family_plugin.inc): the
+    noisemixing = true diffusion VJP of the reference (src/derivative_wrappers.jl:1165-1211) is not built for it.  A
+    general-noise family accepts either value: its diffusion VJP is always the full one, which is what the reference computes
+    with noisemixing = true."""
+    if sensealg is None or not isnoisemixing(sensealg) or family in GENERAL_NOISE_FAMILIES:
         return
     if FAMILIES.get(family, (0, 0, 0))[2] and _lib.FAM.get(family, -1) >= FAM_USER_BASE:
         raise NotImplementedError(f"noisemixing = true: the SDE family plug-in {family!r} is built for diagonal noise that does not "
                                   "mix (g_i depends on u_i and p only)")
+
+
+def _check_general_noise(family, stepper, sensealg):
+    """EM + BacksolveAdjoint integrates the reference's Ito-transformed drift f - J_{vec G}' vec G (src/sde_tools.jl:29-66),
+    which is the Ito correction only for noise that does not mix: it is not built for a general-noise family."""
+    inner = sensealg.inner if isinstance(sensealg, B200Adjoint) else sensealg
+    if family in GENERAL_NOISE_FAMILIES and stepper == "em" and isinstance(inner, BacksolveAdjoint):
+        raise NotImplementedError(f"EM + BacksolveAdjoint is not built for the general-noise SDE family {family!r}: use EulerHeun "
+                                  "or InterpolatingAdjoint")
 
 
 def _check_params(p):
@@ -90,6 +102,7 @@ def adjoint_sensitivities(sol, alg=None, *, sensealg=None, t=None, dgdu_discrete
     if eng is None:
         raise RuntimeError("solution carries no live device handle")
     _check_noise_mixing(eng.family, sensealg)
+    _check_general_noise(eng.family, getattr(sol.alg, "code", None), sensealg)
     ts = sol.t if t is None else np.asarray(t, dtype=np.float64)
     if dgdu_discrete is None:
         ts = np.zeros(0)                                   # continuous cost only: no jumps (discrete = false in the reference)
