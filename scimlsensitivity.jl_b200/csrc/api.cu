@@ -44,30 +44,25 @@ FamilyVTable builtin_sde_family(const char* name) {
     return v;
 }
 constexpr int BUILTIN_FAMILIES = B200ADJ_FAM_RELAX + 1;
-const FamilyVTable* builtin_families() {        // indexed by B200ADJ_FAM_*; abi == 0: the MLP family (own dispatch)
+const FamilyVTable* builtin_families() {        // indexed by B200ADJ_FAM_*
     static const FamilyVTable t[BUILTIN_FAMILIES] = {
         builtin_family<LotkaVolterra, true, true, true>("lv"),
         builtin_family<Lorenz, true, true, true>("lorenz"),
         builtin_family<Robertson, true, true, false>("robertson"),
         builtin_sde_family<SdeLotkaVolterra>("sde_lv"),
-        {},                                     // MLP
+        {B200ADJ_PLUGIN_ABI, MLP_D, MLP_P, "mlp"},      // Path::MLP: mlp_forward_dispatch / mlp_reverse_dispatch
         builtin_sde_family<SdeLinear2>("sde_linear"),
         builtin_family<BouncingBall, false, false, false>("ball"),
         builtin_family<Relax, false, false, false>("relax")};
     return t;
 }
 
-// d, P, m of the families with their own dispatch entry points (mlp_*_dispatch)
-struct FamDims { int32_t id, d, P, m; };
-constexpr FamDims OWN_DISPATCH_FAMILIES[] = {
-    {B200ADJ_FAM_MLP, MLP_D, MLP_P, 0}};
-
 int fam_dims(const b200adj_cfg& c, int* d, int* P, int* m) {
-    if (const FamilyVTable* vt = family_lookup(c.rhs_family)) { *d = vt->d; *P = vt->P; *m = vt->m; return 0; }
     if (c.rhs_family == B200ADJ_FAM_MLP && c.mlp_hidden != MLP_H) return -1;
-    for (const FamDims& f : OWN_DISPATCH_FAMILIES)
-        if (f.id == c.rhs_family) { *d = f.d; *P = f.P; *m = f.m; return 0; }
-    return -1;
+    const FamilyVTable* vt = family_lookup(c.rhs_family);
+    if (!vt) return -1;
+    *d = vt->d; *P = vt->P; *m = vt->m;
+    return 0;
 }
 
 // The support matrix: is `sensealg` built for this execution path, dtype and checkpointing, with preset-time events and a
@@ -235,7 +230,7 @@ void build_hermite_folded(double h, double (*hf)[4]) {
 }
 
 const FamilyVTable* family_lookup(int id) {
-    if (id >= 0 && id < BUILTIN_FAMILIES) { const FamilyVTable* vt = &builtin_families()[id]; return vt->abi ? vt : nullptr; }
+    if (id >= 0 && id < BUILTIN_FAMILIES) return &builtin_families()[id];
     auto& r = family_registry();
     const int k = id - B200ADJ_FAM_USER_BASE_ID;
     return (k >= 0 && k < (int)r.size()) ? r[k] : nullptr;
@@ -300,6 +295,43 @@ T5aArgs t5a_args(Handle* h) {
         a.cc_qcomp = h->cc_qcomp; a.cc_qcoef = h->cc_qcoef;
         a.fe_nc = h->fe_nc; a.cc_ev = h->d_cc_ev;
         for (int c = 0; c < 8; c++) a.fe_dir[c] = h->fe_dir[c];
+    }
+    return a;
+}
+// The arguments of the fixed-step Tsit5 kernels in the real type R.  Preset-time events, the continuous cost and the
+// GaussKronrod tables are F64 only.
+template <class R>
+OdeFwdArgsT<R> fixed_fwd_args(const Handle* h, const void* u0, const void* p, void* saved, int32_t* status) {
+    OdeFwdArgsT<R> a;
+    memset(&a, 0, sizeof(a));
+    a.u0 = (const R*)u0; a.p = (const R*)p; a.ckpt = (R*)h->d_ckpt; a.saved = (R*)saved; a.save_of_step = h->d_fwd_save_of_step;
+    a.status = status; a.N = h->cfg.N; a.Npad = h->Npad; a.S = h->S; a.ckpt_every = h->ckpt_every;
+    if constexpr (std::is_same<R, double>::value) {
+        a.tb = h->tb;
+        a.event_of_step = h->d_event_of_step; a.ev_s = h->d_ev_s; a.ev_c = h->d_ev_c; a.ev_ps = h->d_ev_ps; a.ev_pc = h->d_ev_pc; a.nev = h->nev;
+    } else cast_tables(h->tb, &a.tb);
+    return a;
+}
+template <class R>
+OdeRevArgsT<R> fixed_rev_args(const Handle* h, const void* dLdu, void* du0, void* dp) {
+    const b200adj_cfg& c = h->cfg;
+    OdeRevArgsT<R> a;
+    memset(&a, 0, sizeof(a));
+    a.ckpt = (const R*)h->d_ckpt; a.p = (const R*)h->cur_p; a.dLdu = (const R*)dLdu; a.save_of_step = h->d_save_of_step;
+    a.du0 = (R*)du0; a.dp_members = (R*)dp; a.partials = h->d_partials; a.dp = (R*)dp; a.ticket = h->d_ticket;
+    a.N = c.N; a.Npad = h->Npad; a.S = h->S; a.trace = h->d_trace;
+    for (int j = 0; j < 4; j++) { a.cost_a[j] = (R)h->cost_av[j]; a.cost_b[j] = (R)h->cost_bv[j]; }
+    a.flags = kernel_flags(h);
+    if constexpr (std::is_same<R, double>::value) {
+        a.tb = h->tb;
+        a.event_of_step = h->d_event_of_step; a.ev_s = h->d_ev_s; a.ev_c = h->d_ev_c; a.ev_ps = h->d_ev_ps; a.ev_pc = h->d_ev_pc; a.nev = h->nev;
+        for (int j = 0; j < 4; j++) { a.cont_a[j] = h->cont_av[j]; a.cont_b[j] = h->cont_bv[j]; }
+        tsit5_weights(0.0, nullptr, a.Rpoly); a.hstep = c.dt;
+        build_c4_du_weights(c.dt, a.hC4u);
+        build_hermite_folded(c.dt, a.hHf);
+    } else {
+        cast_tables(h->tb, &a.tb);
+        build_hermite_weights_f32(c.dt, a.hC4u, a.hHf);
     }
     return a;
 }
@@ -786,26 +818,26 @@ int32_t b200adj_event_times(void* handle, int32_t* counts, double* times) {
 
 int32_t b200adj_family_conditions(int32_t family, int32_t* nc) {
     if (!nc) return B200ADJ_ERR_INVALID;
-    if (const FamilyVTable* vt = family_lookup(family)) { *nc = vt->nc; return B200ADJ_OK; }
-    for (const FamDims& f : OWN_DISPATCH_FAMILIES)
-        if (f.id == family) { *nc = 0; return B200ADJ_OK; }
-    return B200ADJ_ERR_INVALID;
+    const FamilyVTable* vt = family_lookup(family);
+    if (!vt) return B200ADJ_ERR_INVALID;
+    *nc = vt->nc;
+    return B200ADJ_OK;
 }
 
 int32_t b200adj_family_noise(int32_t family, int32_t* m) {
     if (!m) return B200ADJ_ERR_INVALID;
-    if (const FamilyVTable* vt = family_lookup(family)) { *m = vt->m; return B200ADJ_OK; }
-    for (const FamDims& f : OWN_DISPATCH_FAMILIES)
-        if (f.id == family) { *m = f.m; return B200ADJ_OK; }
-    return B200ADJ_ERR_INVALID;
+    const FamilyVTable* vt = family_lookup(family);
+    if (!vt) return B200ADJ_ERR_INVALID;
+    *m = vt->m;
+    return B200ADJ_OK;
 }
 
 int32_t b200adj_family_noise_kind(int32_t family, int32_t* kind) {
     if (!kind) return B200ADJ_ERR_INVALID;
-    if (const FamilyVTable* vt = family_lookup(family)) { *kind = vt->noise; return B200ADJ_OK; }
-    for (const FamDims& f : OWN_DISPATCH_FAMILIES)
-        if (f.id == family) { *kind = B200ADJ_NOISE_NONE; return B200ADJ_OK; }
-    return B200ADJ_ERR_INVALID;
+    const FamilyVTable* vt = family_lookup(family);
+    if (!vt) return B200ADJ_ERR_INVALID;
+    *kind = vt->noise;
+    return B200ADJ_OK;
 }
 
 int32_t b200adj_set_family_events(void* handle, int32_t enabled, int32_t nc, const int32_t* direction, int32_t max_events) {
@@ -914,20 +946,10 @@ int32_t b200adj_forward(void* handle, const void* u0, const void* p, const void*
         } else rc = fwd(dense_args<RosArgs>(h), vt->ros_fwd, dstatus);
     } else if (h->path == Path::MLP) {
         rc = mlp_forward_dispatch(h, du0, dp, h->fwd_K > 0 ? dsaved : nullptr, dstatus);
-    } else if (h->path == Path::FIXED && c.dtype == B200ADJ_F32) {
-        OdeFwdArgsT<float> a;
-        memset(&a, 0, sizeof(a));
-        a.u0 = (const float*)du0; a.p = (const float*)dp; a.ckpt = (float*)h->d_ckpt; a.saved = h->fwd_K > 0 ? (float*)dsaved : nullptr;
-        a.save_of_step = h->d_fwd_save_of_step; a.status = dstatus; a.N = c.N; a.Npad = h->Npad; a.S = h->S; a.ckpt_every = h->ckpt_every;
-        cast_tables(h->tb, &a.tb);
-        rc = launch(vt->fwd_f32, h, a);
     } else if (h->path == Path::FIXED) {
-        OdeFwdArgs a;
-        memset(&a, 0, sizeof(a));
-        a.u0 = du0; a.p = dp; a.ckpt = h->d_ckpt; a.saved = h->fwd_K > 0 ? dsaved : nullptr; a.save_of_step = h->d_fwd_save_of_step;
-        a.status = dstatus; a.N = c.N; a.Npad = h->Npad; a.S = h->S; a.tb = h->tb; a.ckpt_every = h->ckpt_every;
-        a.event_of_step = h->d_event_of_step; a.ev_s = h->d_ev_s; a.ev_c = h->d_ev_c; a.ev_ps = h->d_ev_ps; a.ev_pc = h->d_ev_pc; a.nev = h->nev;
-        rc = launch(vt->fwd, h, a);
+        double* sv = h->fwd_K > 0 ? dsaved : nullptr;
+        rc = c.dtype == B200ADJ_F32 ? launch(vt->fwd_f32, h, fixed_fwd_args<float>(h, du0, dp, sv, dstatus))
+                                    : launch(vt->fwd, h, fixed_fwd_args<double>(h, du0, dp, sv, dstatus));
     } else {
         SdeFwdArgs a;
         a.u0 = du0; a.p = dp; a.ckpt = h->d_ckpt; a.saved = h->fwd_K > 0 ? dsaved : nullptr; a.save_of_step = h->d_fwd_save_of_step;
@@ -992,32 +1014,13 @@ int32_t b200adj_reverse(void* handle, const void* dLdu, void* du0, void* dp) {
         rc = mlp_reverse_dispatch(h, dL, ddu0, ddp);
     } else if (h->path == Path::FIXED && c.dtype == B200ADJ_F32) {
         if (h->cont_on) { h->err = "continuous cost: F64 only"; return B200ADJ_ERR_UNSUPPORTED; }
-        OdeRevArgsT<float> a;
-        memset(&a, 0, sizeof(a));
-        a.ckpt = (const float*)h->d_ckpt; a.p = (const float*)h->cur_p; a.dLdu = (const float*)dL; a.save_of_step = h->d_save_of_step;
-        a.du0 = (float*)ddu0; a.dp_members = (float*)ddp; a.partials = h->d_partials; a.dp = (float*)ddp; a.ticket = h->d_ticket;
-        a.N = c.N; a.Npad = h->Npad; a.S = h->S; a.trace = h->d_trace;
-        for (int j = 0; j < 4; j++) { a.cost_a[j] = (float)h->cost_av[j]; a.cost_b[j] = (float)h->cost_bv[j]; }
-        cast_tables(h->tb, &a.tb);
-        build_hermite_weights_f32(c.dt, a.hC4u, a.hHf);
-        a.flags = kernel_flags(h);
-        rc = launch(vt->rev_f32, h, a);
+        rc = launch(vt->rev_f32, h, fixed_rev_args<float>(h, dL, ddu0, ddp));
     } else if (h->path == Path::FIXED) {
-        OdeRevArgs a;
-        memset(&a, 0, sizeof(a));
-        a.event_of_step = h->d_event_of_step; a.ev_s = h->d_ev_s; a.ev_c = h->d_ev_c; a.ev_ps = h->d_ev_ps; a.ev_pc = h->d_ev_pc; a.nev = h->nev;
-        tsit5_weights(0.0, nullptr, a.Rpoly); a.hstep = c.dt;
-        build_c4_du_weights(c.dt, a.hC4u);
-        build_hermite_folded(c.dt, a.hHf);
+        OdeRevArgs a = fixed_rev_args<double>(h, dL, ddu0, ddp);
         if (c.shared_p && comm_fused_ready(h) && !(c.flags & B200ADJ_FLAG_NCCL_ALLREDUCE) && c.sensealg != B200ADJ_SA_QUADRATURE && !h->has_dgdp && !(h->has_cdgdp && h->cont_on)) {
             // the all-reduce of dp is fused into this kernel's last block (peer-memory mailboxes): no collective launch
             a.p2p = h->p2p; a.p2p.epoch = ++h->p2p_epoch; fused_allreduce = true;
         }
-        a.ckpt = h->d_ckpt; a.p = h->cur_p; a.dLdu = dL; a.save_of_step = h->d_save_of_step;
-        a.du0 = ddu0; a.dp_members = ddp; a.partials = h->d_partials; a.dp = ddp; a.ticket = h->d_ticket;
-        a.N = c.N; a.Npad = h->Npad; a.S = h->S; a.tb = h->tb; a.trace = h->d_trace;
-        for (int j = 0; j < 4; j++) { a.cost_a[j] = h->cost_av[j]; a.cost_b[j] = h->cost_bv[j]; a.cont_a[j] = h->cont_av[j]; a.cont_b[j] = h->cont_bv[j]; }
-        a.flags = kernel_flags(h);
         rc = launch(vt->rev, h, a);
     } else {
         SdeRevArgs a;

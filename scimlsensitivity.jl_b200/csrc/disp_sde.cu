@@ -8,8 +8,6 @@ template int launch_sde_fwd<SdeLinear2>(Handle*, const SdeFwdArgs&);
 template int launch_sde_rev<SdeLinear2>(Handle*, const SdeRevArgs&);
 
 int sde_noise_launch(Handle* h, const SdeNoiseArgs& a, int64_t total) {
-    sde_noise_kernel<0><<<(unsigned)((total + 255) / 256), 256, 0, h->stream>>>(a);
-    h->launches++;
-    return 0;
+    return launch_kernel(h, sde_noise_kernel<0>, (unsigned)((total + 255) / 256), 256, 0, a);
 }
 }  // namespace b200adj

@@ -10,6 +10,7 @@
 #include <stdlib.h>
 
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "../../include/b200adj.h"
@@ -110,6 +111,33 @@ struct Handle {
         }                                                                                      \
     } while (0)
 
+// ---- kernel dispatch (disp_*): a runtime choice becomes a std::integral_constant passed to the generic lambda f, whose
+// body names the kernel instantiation with X.value ----
+template <class F> int with_flag(bool b, F&& f) { return b ? f(std::true_type{}) : f(std::false_type{}); }
+template <class F> int with_cost(const Handle* h, F&& f) {
+    if (h->cfg.cost_kind == B200ADJ_COST_EXPLICIT) return f(std::integral_constant<int, COST_EXPLICIT>{});
+    return f(std::integral_constant<int, COST_AFFINE>{});
+}
+template <class F> int with_sensealg(int32_t sensealg, F&& f) {
+    switch (sensealg) {
+    case B200ADJ_SA_INTERPOLATING: return f(std::integral_constant<int, SA_INTERP>{});
+    case B200ADJ_SA_GAUSS: return f(std::integral_constant<int, SA_GAUSS>{});
+    case B200ADJ_SA_BACKSOLVE: return f(std::integral_constant<int, SA_BACKSOLVE>{});
+    case B200ADJ_SA_GAUSSKRONROD: return f(std::integral_constant<int, SA_GK>{});
+    case B200ADJ_SA_QUADRATURE: return f(std::integral_constant<int, SA_QUAD>{});
+    default: return B200ADJ_ERR_UNSUPPORTED;
+    }
+}
+// One launch on the handle's stream.  Static shared memory rides on top of the dynamic `smem`, so the kernel opts in to
+// more dynamic shared memory well below the 48 KB default limit.
+template <class... P, class... A>
+int launch_kernel(Handle* h, void (*kernel)(P...), dim3 grid, dim3 block, size_t smem, const A&... args) {
+    if (smem > 30 * 1024 && cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return B200ADJ_ERR_CUDA;
+    kernel<<<grid, block, smem, h->stream>>>(args...);
+    h->launches++;
+    return 0;
+}
+
 inline bool is_sde(const b200adj_cfg& c) { return c.stepper == B200ADJ_ST_EM || c.stepper == B200ADJ_ST_EULER_HEUN; }
 inline bool is_adaptive(const Handle* h) { return h->path == Path::T5A || h->path == Path::ROS; }
 // T5A run with a constant step and no error control (fixed-step Tsit5 with off-grid save times)
@@ -155,7 +183,8 @@ template <class T, class S> inline void cast_tables(const S& src, T* dst) {
 // gvjp_p_apply of its D x M diffusion with the increments; sde_em.cuh);
 // the plug-in instantiates the same kernel templates for it and exports this table of launchers (family_plugin.inc).
 // b200adj_register_family(path) loads it and hands out a family id >= B200ADJ_FAM_USER_BASE.  The built-in families fill
-// the same table (api.cu, builtin_families), so every family but MLP dispatches through one lookup. ----
+// the same table (api.cu, builtin_families), so every family dispatches through one lookup (the MLP family's row has no
+// launchers: Path::MLP has its own, mlp_*_dispatch). ----
 struct FamilyVTable {
     uint32_t abi;                 // B200ADJ_PLUGIN_ABI of the headers the plug-in was built from
     int32_t d, P;
@@ -178,7 +207,7 @@ constexpr uint32_t B200ADJ_PLUGIN_ABI = 0x00030000u ^ (uint32_t)sizeof(Handle) ^
                                         ((uint32_t)sizeof(T5aArgs) << 16) ^ ((uint32_t)sizeof(FamilyVTable) << 24) ^
                                         ((uint32_t)sizeof(SdeFwdArgs) << 4) ^ ((uint32_t)sizeof(SdeRevArgs) << 12);
 constexpr int B200ADJ_FAM_USER_BASE_ID = 100;
-// api.cu: the ODE and SDE families, built-in (id < B200ADJ_FAM_USER_BASE_ID) and registered plug-ins; null for the MLP family
+// api.cu: the families, built-in (id < B200ADJ_FAM_USER_BASE_ID) and registered plug-ins; null for an unknown id
 const FamilyVTable* family_lookup(int id);
 
 // ---- dispatch entry points, one explicit instantiation per family in disp_*.cu ----
@@ -212,5 +241,22 @@ template <class K> inline int quad_launch_grid(const Handle* h, K kernel, size_t
 int ensure_quad_buffers(Handle* h);      // api.cu: lazily allocates QuadratureAdjoint's dense solutions and the quadgk scratch
 inline size_t quad_smem(int maxseg) { return (size_t)QUAD_WARPS * (QUAD_SKEYS + quad_l1_blocks(maxseg)) * sizeof(double); }
 inline size_t quad_seg_doubles(int P, int maxseg, int qgrid) { return (size_t)qgrid * QUAD_WARPS * maxseg * (size_t)(((P + 4 + 3) / 4) * 4); }
+// QuadratureAdjoint on every stepper: its buffers, then `rev` (the stepper's SA_QUAD reverse pass, which stores the dense
+// reverse solution; on Rosenbrock23 also the member-major copy of the forward one), then the quadrature kernel kernel(SP)
+// over the persistent grid with the arguments args(), taken once the buffers exist
+template <class Rev, class Kernel, class Args>
+int quadrature_adjoint(Handle* h, Rev&& rev, Kernel&& kernel, Args&& args) {
+    if (int rc = ensure_quad_buffers(h)) return rc;
+    if (int rc = rev()) return rc;
+    if ((size_t)h->qgrid > h->qpartials_blocks) return B200ADJ_ERR_INVALID;
+    const auto a = args();
+    const size_t smem = quad_smem(h->maxseg);
+    return with_flag(h->cfg.shared_p, [&](auto SP) {
+        const auto k = kernel(SP);
+        k<<<quad_launch_grid(h, k, smem), QUAD_WARPS * 32, smem, h->stream>>>(a);
+        h->launches++;
+        return 0;
+    });
+}
 
 }  // namespace b200adj
