@@ -1,5 +1,6 @@
 // wgmma_probe.cu -- one-CTA probes of the tensor-core building blocks of the bf16 neural-ODE kernels (csrc/wgmma.cuh,
-// csrc/mlp_tc.cuh, csrc/mlp_tc_wide.cuh), for tests/test_gpu_wgmma_probe.py.  The production device functions are called
+// csrc/mlp_tc.cuh, csrc/mlp_tc_wide.cuh), for tests/test_gpu_wgmma_probe.py, and the element-wise tanh_fast / pack_bf16 for the
+// bf16 twin of tests/test_gpu_mlp_bf16_reference.py.  The production device functions are called
 // unchanged; this file only adds __global__ wrappers and extern "C" launchers over device pointers.  Test-only: it is not
 // part of libb200adj.so.
 //
@@ -122,6 +123,25 @@ __global__ void __launch_bounds__(TCW_M) tcw_stage_probe(const float* p, const f
     tc_grad_store(g, partial);
 }
 
+// ---- the element-wise device functions the bf16 twin of tests/mlp_bf16_twin.py restates: tanh_fast (tanh.approx.f32)
+// and pack_bf16 (two fp32 -> one bf16x2 word, first argument in the low half)
+__global__ void tanh_probe(const float* x, float* y, int64_t n) {
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) y[i] = tanh_fast(x[i]);
+}
+__global__ void pack_probe(const float* x, uint32_t* out, int64_t npairs) {
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < npairs; i += (int64_t)gridDim.x * blockDim.x)
+        out[i] = pack_bf16(x[2 * i], x[2 * i + 1]);
+}
+template <class K, class... A>
+int launch_elementwise(K kernel, int64_t n, A... args) {
+    if (n <= 0) return 0;
+    const int grid = (int)((n + 255) / 256 < 4096 ? (n + 255) / 256 : 4096);
+    kernel<<<grid, 256>>>(args..., n);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return (int)e;
+    return (int)cudaDeviceSynchronize();
+}
+
 template <class S, class K, class... A>
 int launch(K kernel, A... args) {
     const int smem = (int)sizeof(S) + 128;
@@ -148,3 +168,7 @@ extern "C" int probe_stage(int wide, const float* p, const float* y, const float
     return wide ? launch<TcwSmem>(tcw_stage_probe, p, y, L, valid, wt, F, J, partial)
                 : launch<TcSmem>(tc_stage_probe, p, y, L, valid, wt, F, J, partial);
 }
+// y[i] = tanh_fast(x[i]), i < n
+extern "C" int probe_tanh_approx(const float* x, float* y, int64_t n) { return launch_elementwise(tanh_probe, n, x, y); }
+// out[i] = pack_bf16(x[2 i], x[2 i + 1]), i < npairs
+extern "C" int probe_pack_bf16(const float* x, uint32_t* out, int64_t npairs) { return launch_elementwise(pack_probe, npairs, x, out); }

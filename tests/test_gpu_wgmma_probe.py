@@ -46,7 +46,7 @@ def test_probe_compiles_for_sm90a(probe_so):
     """No GPU needed: a header change that breaks the probes fails here."""
     assert os.path.getsize(probe_so) > 0
     lib = C.CDLL(probe_so)
-    for name in ("probe_member_gemm", "probe_grad_gemm", "probe_stage"):
+    for name in ("probe_member_gemm", "probe_grad_gemm", "probe_stage", "probe_tanh_approx", "probe_pack_bf16"):
         getattr(lib, name)
 
 
