@@ -81,8 +81,10 @@ enum { B200ADJ_COST_EXPLICIT = 0, B200ADJ_COST_AFFINE = 1 };
                                               /* has off-grid entries; set it to re-target the reverse pass to off-grid times later)  */
 #define B200ADJ_FLAG_NCCL_ALLREDUCE    128u   /* multi-GPU: sum dp with ncclAllReduce instead of the all-reduce fused into the reverse    */
                                               /* kernel over peer-memory mailboxes (the default whenever the GPUs can map each other)    */
+#define B200ADJ_FLAG_CHECKPOINT_SAVES  256u   /* adaptive Tsit5: checkpointed save intervals (see checkpoint_every below) */
 /* flags fixed at create (the others can be changed per reverse pass by b200adj_set_reverse_options) */
-#define B200ADJ_CREATE_FLAGS (B200ADJ_FLAG_STORED_NOISE | B200ADJ_FLAG_TRACE | B200ADJ_FLAG_NO_ROTATE | B200ADJ_FLAG_DENSE_FORWARD | B200ADJ_FLAG_NCCL_ALLREDUCE)
+#define B200ADJ_CREATE_FLAGS (B200ADJ_FLAG_STORED_NOISE | B200ADJ_FLAG_TRACE | B200ADJ_FLAG_NO_ROTATE | B200ADJ_FLAG_DENSE_FORWARD | B200ADJ_FLAG_NCCL_ALLREDUCE | \
+                              B200ADJ_FLAG_CHECKPOINT_SAVES)
 
 /* error codes */
 #define B200ADJ_OK                 0
@@ -111,11 +113,20 @@ typedef struct b200adj_cfg {
     int32_t checkpoint_every;        /* fixed-step Tsit5: keep the forward state every C steps only; the reverse pass re-solves each */
                                      /* C-step segment into shared memory (CheckpointSolution, src/interpolating_adjoint.jl:54-112,  */
                                      /* 206-278; src/gauss_adjoint.jl:57-95, 167-212).  0 or 1 = every step                          */
+                                     /* The adaptive Tsit5 stepper checkpoints with B200ADJ_FLAG_CHECKPOINT_SAVES instead: the forward */
+                                     /* pass keeps, per member and save interval, only the step state (t_n, u_n, f(u_n), first-attempt */
+                                     /* step size, qold) of the step that holds the interval's lower bound; the reverse pass re-solves */
+                                     /* one interval at a time and gets the gradient of the full dense solution bit for bit.  The      */
+                                     /* intervals are bounded by t0, the save times inside (t0, t1) and t1.  Interpolating / Gauss /   */
+                                     /* GaussKronrod, no events or continuous callbacks, and the reverse pass keeps the forward save   */
+                                     /* times (everything else is B200ADJ_ERR_UNSUPPORTED).  max_steps then sizes ONE interval.        */
     uint32_t flags;
     int32_t mlp_hidden;              /* FAM_MLP hidden width                                               */
     int32_t block_threads;           /* 0 = library default; tuning knob                                   */
     int32_t max_steps;               /* adaptive steppers: per-member step capacity of the dense forward / reverse solutions */
-                                     /* (the reference's maxiters); 0 = 4096                                */
+                                     /* (the reference's maxiters); 0 = 4096.  With B200ADJ_FLAG_CHECKPOINT_SAVES: the accepted */
+                                     /* steps of ONE save interval (pass the longest interval's count); a member that needs more */
+                                     /* gets status 2 and NaN gradients, the total is bounded by the iteration cap only          */
     int32_t reserved0;               /* must be 0                                                          */
 } b200adj_cfg;
 
@@ -264,6 +275,13 @@ int32_t b200adj_set_stream(void* handle, void* cuda_stream);
 int32_t b200adj_synchronize(void* handle);
 /* number of kernels this handle has launched so far (bench.py's gpu_launches) */
 int64_t b200adj_launch_count(void* handle);
+/* device memory the handle owns at the time of the call, in bytes (every buffer it allocated and has not freed yet: dense
+ * solutions or checkpoints, save tables, staging, lazily allocated QuadratureAdjoint and event buffers).  For an adaptive
+ * Tsit5 handle with buffers_on_device = 1 and no events:
+ *   N (MS+1) (8 d + 5) 8  +  12 N  +  2 max(K,1) 8  +  max(qgrid+1, ceil(N/32)) P 8  +  4
+ *   [+ N n_seg (2 d + 4) 8 with B200ADJ_FLAG_CHECKPOINT_SAVES, n_seg = 1 + the save times inside (t0, t1)]
+ * with MS = max_steps (0: 4096) and qgrid = min(ceil(N / 4), 6 n_SM).  Sizes ensembles before they run out of memory. */
+int32_t b200adj_device_bytes(void* handle, int64_t* bytes);
 /* adaptive steppers: per-member accepted step counts of the last forward / reverse solves (device or host per cfg) */
 int32_t b200adj_get_step_counts(void* handle, int32_t* fwd_steps, int32_t* rev_steps);
 

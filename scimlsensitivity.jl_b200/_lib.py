@@ -19,11 +19,12 @@ ST = {"tsit5_fixed": 0, "rosenbrock23": 1, "em": 2, "euler_heun": 3, "tsit5_adap
 DTYPE = {"f64": 0, "f32": 1, "bf16_f32acc": 2}
 COST = {"explicit": 0, "affine": 1}
 FLAG_NO_START, FLAG_NO_CHECKPOINTING, FLAG_CKPT_EVERY_STEP, FLAG_STORED_NOISE, FLAG_TRACE, FLAG_NO_ROTATE, FLAG_DENSE_FORWARD, FLAG_NCCL_ALLREDUCE = 1, 2, 4, 8, 16, 32, 64, 128
+FLAG_CHECKPOINT_SAVES = 256        # adaptive Tsit5: checkpointed save intervals, re-solved one at a time by the reverse pass
 NOISE_NONE, NOISE_DIAGONAL, NOISE_GENERAL = 0, 1, 2
 ERR = {0: "OK", -1: "INVALID", -2: "UNSUPPORTED", -3: "NO_DEVICE", -4: "CUDA", -5: "STATE", -6: "OOM"}
 
 EXPORTS = ["b200adj_create", "b200adj_forward", "b200adj_reverse", "b200adj_set_reverse_options", "b200adj_set_tolerances", "b200adj_set_continuous_cost", "b200adj_set_cost_family", "b200adj_register_family", "b200adj_family_info", "b200adj_set_events", "b200adj_set_event_param_shift", "b200adj_set_continuous_callback", "b200adj_set_continuous_callback_params", "b200adj_event_times", "b200adj_family_conditions", "b200adj_family_noise", "b200adj_family_noise_kind", "b200adj_set_family_events", "b200adj_event_flags", "b200adj_get_noise", "b200adj_set_stream",
-           "b200adj_synchronize", "b200adj_launch_count", "b200adj_get_step_counts", "b200adj_get_block_trace", "b200adj_destroy",
+           "b200adj_synchronize", "b200adj_launch_count", "b200adj_device_bytes", "b200adj_get_step_counts", "b200adj_get_block_trace", "b200adj_destroy",
            "b200adj_last_error", "b200adj_version", "b200adj_sizeof_cfg",
            "b200adj_comm_unique_id", "b200adj_comm_init", "b200adj_comm_init_all", "b200adj_comm_allreduce", "b200adj_comm_size", "b200adj_comm_is_fused"]
 
@@ -169,6 +170,8 @@ def load():
         lib.b200adj_synchronize.restype = C.c_int32
         lib.b200adj_launch_count.argtypes = [C.c_void_p]
         lib.b200adj_launch_count.restype = C.c_int64
+        lib.b200adj_device_bytes.argtypes = [C.c_void_p, C.POINTER(C.c_int64)]
+        lib.b200adj_device_bytes.restype = C.c_int32
         lib.b200adj_get_step_counts.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
         lib.b200adj_get_step_counts.restype = C.c_int32
         lib.b200adj_get_block_trace.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(C.c_int32)]
@@ -409,6 +412,12 @@ class Handle:
     @property
     def launch_count(self):
         return int(self._lib.b200adj_launch_count(self._h))
+
+    def device_bytes(self):
+        """Device memory the handle owns now, in bytes."""
+        n = C.c_int64()
+        self._check(self._lib.b200adj_device_bytes(self._h, C.byref(n)))
+        return n.value
 
     def close(self):
         if self._h:

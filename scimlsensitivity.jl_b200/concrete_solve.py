@@ -167,12 +167,13 @@ def solve(eprob, alg, ensemblealg=None, *, trajectories=None, saveat=None, sense
     block = getattr(sensealg, "block_threads", 0) if isinstance(sensealg, B200Adjoint) else 0
     stored = getattr(sensealg, "stored_noise", False) if isinstance(sensealg, B200Adjoint) else False
     ckpt_every = getattr(sensealg, "checkpoint_every", 1) if isinstance(sensealg, B200Adjoint) else 1
+    ckpt_saves = bool(getattr(sensealg, "checkpoint_saves", False)) if isinstance(sensealg, B200Adjoint) else False
     ev = callback.tables(d, P) if callback is not None else None
     evp = callback.param_shift() if callback is not None else None
     key = (prob.f, alg.code, hi - lo, ts.tobytes(), tuple(prob.tspan), _step_size(alg, kwargs), shared_p, on_device, device,
            getattr(prob, "seed", 0), lo, block, stored, ckpt_every, kwargs.get("abstol", 1e-6), kwargs.get("reltol", 1e-3),
            None if ev is None else tuple(x.tobytes() for x in ev), None if evp is None else tuple(x.tobytes() for x in evp),
-           None if ccb is None else ccb.key())
+           None if ccb is None else ccb.key(), ckpt_saves)
     eng = _HANDLE_CACHE.get(key) if ensemblealg.reuse_handle else None
     if eng is None:
         eng = DeviceEnsemble(prob.f, sensealg_name(inner), alg.code, hi - lo, ts, prob.tspan, _step_size(alg, kwargs),
@@ -181,7 +182,7 @@ def solve(eprob, alg, ensemblealg=None, *, trajectories=None, saveat=None, sense
                              quad_abstol=getattr(inner, "abstol", 1e-6), quad_reltol=getattr(inner, "reltol", 1e-3),
                              abstol=kwargs.get("abstol", 1e-6), reltol=kwargs.get("reltol", 1e-3),
                              max_steps=kwargs.get("maxiters", 0), pin_outputs=ensemblealg.pin_outputs,
-                             checkpoint_every=ckpt_every)
+                             checkpoint_every=ckpt_every, checkpoint_saves=ckpt_saves)
         if ev is not None:
             eng.set_events(*ev)
             if evp is not None:

@@ -75,7 +75,8 @@ enum SupportRules : unsigned {
     SR_SENSEALG = 4,       // SDE: Backsolve / Interpolating; known sensealg; GaussKronrod F64 only
     SR_CKPT = 8,           // checkpoint_every > 1: fixed-step Tsit5 with Interpolating / Gauss
     SR_CALLBACKS = 16,     // QuadratureAdjoint: no events, no continuous callback
-    SR_ALL = 31
+    SR_CKSAVES = 32,       // B200ADJ_FLAG_CHECKPOINT_SAVES: adaptive Tsit5, Interpolating / Gauss / GaussKronrod, no callbacks
+    SR_ALL = 63
 };
 int32_t check_support(const b200adj_cfg& c, Path path, int ckpt_every, int32_t sensealg, bool events, bool callback, std::string& err,
                       unsigned rules = SR_ALL) {
@@ -99,6 +100,14 @@ int32_t check_support(const b200adj_cfg& c, Path path, int ckpt_every, int32_t s
         return refuse("checkpoint_every > 1: fixed-step Tsit5 with InterpolatingAdjoint / GaussAdjoint (the sensealgs that checkpoint in the reference)");
     if ((rules & SR_CALLBACKS) && sensealg == B200ADJ_SA_QUADRATURE && events) return refuse("events: QuadratureAdjoint has no callback support");
     if ((rules & SR_CALLBACKS) && sensealg == B200ADJ_SA_QUADRATURE && callback) return refuse("continuous callback: QuadratureAdjoint has no callback support");
+    if ((rules & SR_CKSAVES) && (c.flags & B200ADJ_FLAG_CHECKPOINT_SAVES)) {
+        if (path != Path::T5A || c.stepper != B200ADJ_ST_TSIT5_ADAPTIVE)
+            return refuse("B200ADJ_FLAG_CHECKPOINT_SAVES: built for the adaptive Tsit5 stepper (not Rosenbrock23, the fixed step grid, SDE or MLP)");
+        if (sensealg != B200ADJ_SA_INTERPOLATING && sensealg != B200ADJ_SA_GAUSS && sensealg != B200ADJ_SA_GAUSSKRONROD)
+            return refuse("B200ADJ_FLAG_CHECKPOINT_SAVES: Interpolating / Gauss / GaussKronrod are built (Backsolve and Quadrature need every forward knot)");
+        if (events) return refuse("B200ADJ_FLAG_CHECKPOINT_SAVES: events together with checkpointed save intervals are not built");
+        if (callback) return refuse("B200ADJ_FLAG_CHECKPOINT_SAVES: a continuous callback together with checkpointed save intervals is not built");
+    }
     return B200ADJ_OK;
 }
 int32_t check_support(Handle* h, int32_t sensealg, bool events, bool callback) {
@@ -106,8 +115,8 @@ int32_t check_support(Handle* h, int32_t sensealg, bool events, bool callback) {
 }
 
 // a device copy of a host table, at least one element long so that the pointer is valid for an empty table
-template <class T> cudaError_t upload_table(T** dst, const T* src, size_t n) {
-    cudaError_t e = cudaMalloc(dst, (n > 0 ? n : 1) * sizeof(T));
+template <class T> cudaError_t upload_table(Handle* h, T** dst, const T* src, size_t n) {
+    cudaError_t e = dev_malloc(h, dst, (n > 0 ? n : 1) * sizeof(T));
     if (e == cudaSuccess && n > 0) e = cudaMemcpy(*dst, src, n * sizeof(T), cudaMemcpyHostToDevice);
     return e;
 }
@@ -117,7 +126,7 @@ cudaError_t alloc_staging(Handle* h) {
     const b200adj_cfg& c = h->cfg;
     const size_t N = (size_t)c.N, e = esz(c), dn = (size_t)c.d * N, pn = c.shared_p ? (size_t)c.P : (size_t)c.P * N;
     cudaError_t r = cudaSuccess;
-    auto get = [&](auto** p, size_t bytes) { if (r == cudaSuccess) r = cudaMalloc(p, bytes); };
+    auto get = [&](auto** p, size_t bytes) { if (r == cudaSuccess) r = dev_malloc(h, p, bytes); };
     get(&h->s_u0, dn * e); get(&h->s_p, pn * e); get(&h->s_du0, dn * e); get(&h->s_dp, pn * e); get(&h->s_status, N * sizeof(int32_t));
     if (c.K > 0) {
         get(&h->s_saved, (size_t)c.K * dn * e);
@@ -242,7 +251,7 @@ const FamilyVTable* family_lookup(int id) {
 int ensure_quad_buffers(Handle* h) {
     const b200adj_cfg& c = h->cfg;
     const size_t N = (size_t)c.N, MS = (size_t)h->maxs;
-    auto get = [](double** p, size_t n) { return *p || cudaMalloc(p, n * sizeof(double)) == cudaSuccess; };
+    auto get = [&](double** p, size_t n) { return *p || dev_malloc(h, p, n * sizeof(double)) == cudaSuccess; };
     bool ok;
     if (h->path == Path::FIXED) {
         ok = get(&h->d_adj_dense, (size_t)h->S * 8 * c.d * (size_t)h->Npad);
@@ -282,6 +291,7 @@ T5aArgs t5a_args(Handle* h) {
     T5aArgs a = dense_args<T5aArgs>(h);
     a.dt0 = h->cfg.dt;
     a.status = h->r_status;
+    a.ck = h->d_ck; a.ck_nseg = h->ck_nseg; a.ck_k0 = h->ck_k0; a.ck_abstol = h->cfg.abstol; a.ck_reltol = h->cfg.reltol;
     memcpy(a.A, TSIT5_A, sizeof(TSIT5_A)); memcpy(a.C, TSIT5_C, sizeof(TSIT5_C)); memcpy(a.BT, TSIT5_BT, sizeof(TSIT5_BT));
     tsit5_weights(0.0, nullptr, a.R);
     if (h->cont_on) for (int j = 0; j < 4; j++) { a.cont_a[j] = h->cont_av[j]; a.cont_b[j] = h->cont_bv[j]; }
@@ -340,12 +350,12 @@ template <class A> int launch(int (*fn)(Handle*, const A&), Handle* h, const A& 
 
 void free_all(Handle* h) {
     cudaSetDevice(h->cfg.device);
-    cudaFree(h->r_ft); cudaFree(h->r_fu); cudaFree(h->r_fk); cudaFree(h->r_rrec); cudaFree(h->r_rend); cudaFree(h->r_ftT); cudaFree(h->r_frecT);
-    cudaFree(h->d_saveat); cudaFree(h->r_fn); cudaFree(h->r_rn); cudaFree(h->r_qseg); cudaFree(h->r_qkey);
-    cudaFree(h->d_kst); cudaFree(h->d_adj_dense); cudaFree(h->d_trace); cudaFree(h->d_ckpt); cudaFree(h->d_noise); cudaFree(h->d_partials); cudaFree(h->d_ticket); cudaFree(h->d_save_of_step); cudaFree(h->d_fwd_save_of_step); cudaFree(h->d_fwd_saveat);
-    cudaFree(h->s_u0); cudaFree(h->s_p); cudaFree(h->s_saved); cudaFree(h->s_dLdu); cudaFree(h->s_du0); cudaFree(h->s_dp); cudaFree(h->s_dW);
-    cudaFree(h->d_cc_t); cudaFree(h->d_cc_n); cudaFree(h->d_cc_ev);
-    cudaFree(h->s_status); cudaFree(h->r_status); cudaFree(h->d_event_of_step); cudaFree(h->d_ev_ac); cudaFree(h->d_ev_ak); cudaFree(h->d_ev_af); cudaFree(h->d_ev_t); cudaFree(h->d_ev_s); cudaFree(h->d_ev_c); cudaFree(h->d_ev_ps); cudaFree(h->d_ev_pc);
+    dev_free(h, h->r_ft); dev_free(h, h->r_fu); dev_free(h, h->r_fk); dev_free(h, h->r_rrec); dev_free(h, h->r_rend); dev_free(h, h->r_ftT); dev_free(h, h->r_frecT);
+    dev_free(h, h->d_saveat); dev_free(h, h->r_fn); dev_free(h, h->r_rn); dev_free(h, h->r_qseg); dev_free(h, h->r_qkey);
+    dev_free(h, h->d_kst); dev_free(h, h->d_adj_dense); dev_free(h, h->d_trace); dev_free(h, h->d_ckpt); dev_free(h, h->d_noise); dev_free(h, h->d_partials); dev_free(h, h->d_ticket); dev_free(h, h->d_save_of_step); dev_free(h, h->d_fwd_save_of_step); dev_free(h, h->d_fwd_saveat);
+    dev_free(h, h->s_u0); dev_free(h, h->s_p); dev_free(h, h->s_saved); dev_free(h, h->s_dLdu); dev_free(h, h->s_du0); dev_free(h, h->s_dp); dev_free(h, h->s_dW);
+    dev_free(h, h->d_cc_t); dev_free(h, h->d_cc_n); dev_free(h, h->d_cc_ev); dev_free(h, h->d_ck);
+    dev_free(h, h->s_status); dev_free(h, h->r_status); dev_free(h, h->d_event_of_step); dev_free(h, h->d_ev_ac); dev_free(h, h->d_ev_ak); dev_free(h, h->d_ev_af); dev_free(h, h->d_ev_t); dev_free(h, h->d_ev_s); dev_free(h, h->d_ev_c); dev_free(h, h->d_ev_ps); dev_free(h, h->d_ev_pc);
     if (h->own_stream) cudaStreamDestroy(h->own_stream);
 }
 
@@ -353,16 +363,16 @@ void free_all(Handle* h) {
 int32_t cc_lists(Handle* h, int32_t max_events) {
     const size_t N = (size_t)h->cfg.N, E = (size_t)max_events;
     if (E != (size_t)h->cc_maxev || !h->d_cc_ev) {      // (cc_ev is allocated last: set only when all three are)
-        cudaFree(h->d_cc_t); cudaFree(h->d_cc_n); cudaFree(h->d_cc_ev); h->d_cc_t = nullptr; h->d_cc_n = nullptr; h->d_cc_ev = nullptr; h->cc_on = false;
-        CUDA_TRY(h, cudaMalloc(&h->d_cc_t, E * N * sizeof(double)));
-        CUDA_TRY(h, cudaMalloc(&h->d_cc_n, N * sizeof(int32_t)));
-        CUDA_TRY(h, cudaMalloc(&h->d_cc_ev, E * N * sizeof(int32_t)));
+        dev_free(h, h->d_cc_t); dev_free(h, h->d_cc_n); dev_free(h, h->d_cc_ev); h->d_cc_t = nullptr; h->d_cc_n = nullptr; h->d_cc_ev = nullptr; h->cc_on = false;
+        CUDA_TRY(h, dev_malloc(h, &h->d_cc_t, E * N * sizeof(double)));
+        CUDA_TRY(h, dev_malloc(h, &h->d_cc_n, N * sizeof(int32_t)));
+        CUDA_TRY(h, dev_malloc(h, &h->d_cc_ev, E * N * sizeof(int32_t)));
     }
     CUDA_TRY(h, cudaMemsetAsync(h->d_cc_n, 0, N * sizeof(int32_t), h->stream));
     return B200ADJ_OK;
 }
 void cc_release(Handle* h) {
-    cudaFree(h->d_cc_t); cudaFree(h->d_cc_n); cudaFree(h->d_cc_ev); h->d_cc_t = nullptr; h->d_cc_n = nullptr; h->d_cc_ev = nullptr;
+    dev_free(h, h->d_cc_t); dev_free(h, h->d_cc_n); dev_free(h, h->d_cc_ev); h->d_cc_t = nullptr; h->d_cc_n = nullptr; h->d_cc_ev = nullptr;
     h->cc_on = false; h->fe_nc = 0; h->have_forward = false;
 }
 
@@ -443,6 +453,7 @@ int32_t b200adj_create(const b200adj_cfg* cfg, void** handle) {
     if (sde && m == 0) { g_create_error = "SDE stepper needs an SDE family"; return B200ADJ_ERR_INVALID; }
     if (!sde && m != 0) { g_create_error = "ODE stepper with an SDE family"; return B200ADJ_ERR_INVALID; }
     if (int32_t rc = support(SR_SENSEALG)) return rc;
+    if (int32_t rc = support(SR_CKSAVES)) return rc;
     if (!sde && cfg->stepper != B200ADJ_ST_TSIT5_FIXED && !ros) { g_create_error = "stepper not built on device yet"; return B200ADJ_ERR_UNSUPPORTED; }
     if (ros && !dense_fixed && !(cfg->abstol > 0 && cfg->reltol > 0)) { g_create_error = "adaptive steppers need abstol, reltol > 0"; return B200ADJ_ERR_INVALID; }
     if (cfg->rhs_family == B200ADJ_FAM_RELAX && !t5a) { g_create_error = "Relax family: Tsit5 on the per-member dense framework (adaptive, or fixed step with B200ADJ_FLAG_DENSE_FORWARD)"; return B200ADJ_ERR_UNSUPPORTED; }
@@ -458,7 +469,7 @@ int32_t b200adj_create(const b200adj_cfg* cfg, void** handle) {
             if (cfg->saveat[k] < cfg->t0 || cfg->saveat[k] > cfg->t1 || (k > 0 && !(cfg->saveat[k] > cfg->saveat[k - 1]))) {
                 g_create_error = "saveat must be ascending inside [t0, t1]"; return B200ADJ_ERR_INVALID; }
         }
-        maxs = cfg->max_steps > 0 ? cfg->max_steps : 4096;      // per-member step capacity (forward and dense reverse)
+        maxs = cfg->max_steps > 0 ? cfg->max_steps : 4096;      // per-member step capacity (forward and dense reverse; checkpointed: one save interval)
         if (dense_fixed) {
             // constant step: S forward steps; the reverse solve adds at most one clipped step per tstop (save times, events)
             const long long S_ = llround((cfg->t1 - cfg->t0) / cfg->dt);
@@ -528,43 +539,53 @@ int32_t b200adj_create(const b200adj_cfg* cfg, void** handle) {
     const size_t N = (size_t)cfg->N, e = esz(*cfg);
     // the forward pass keeps its own save table: set_reverse_options may re-target the reverse pass' jump times
     h->fwd_K = cfg->K; h->fwd_saveat = h->saveat;
-    CREATE_TRY(upload_table(&h->d_saveat, cfg->saveat, (size_t)cfg->K));
+    CREATE_TRY(upload_table(h, &h->d_saveat, cfg->saveat, (size_t)cfg->K));
     if (ros) {
         const size_t MS = (size_t)maxs;
         if (t5a) {      // member-major records (u_n, k1..k7, t_n, h, 1/h, t_{n+1}) and knots: tsit5_adaptive.cuh
-            CREATE_TRY(cudaMalloc(&h->r_ftT, N * (MS + 1) * e));
-            CREATE_TRY(cudaMalloc(&h->r_frecT, N * (MS + 1) * (size_t)(8 * d + 4) * e));
-            CREATE_TRY(cudaMalloc(&h->r_status, N * sizeof(int32_t)));
+            // (checkpointed save intervals: the records of ONE interval, re-solved by the reverse kernel, and the intervals' checkpoints)
+            CREATE_TRY(dev_malloc(h, &h->r_ftT, N * (MS + 1) * e));
+            CREATE_TRY(dev_malloc(h, &h->r_frecT, N * (MS + 1) * (size_t)(8 * d + 4) * e));
+            CREATE_TRY(dev_malloc(h, &h->r_status, N * sizeof(int32_t)));
+            if (cfg->flags & B200ADJ_FLAG_CHECKPOINT_SAVES) {
+                int k0 = 0, inner = 0;
+                for (int k = 0; k < cfg->K; k++) {
+                    if (cfg->saveat[k] <= cfg->t0) k0 = k + 1;
+                    else if (cfg->saveat[k] < cfg->t1) inner++;
+                }
+                h->ck_k0 = k0; h->ck_nseg = inner + 1;
+                CREATE_TRY(dev_malloc(h, &h->d_ck, N * (size_t)h->ck_nseg * (size_t)(2 * d + 4) * sizeof(double)));
+            }
         } else {        // Rosenbrock23: step-major knots, states and the 2 dense-output stages
-            CREATE_TRY(cudaMalloc(&h->r_ft, (MS + 1) * N * e));
-            CREATE_TRY(cudaMalloc(&h->r_fu, (MS + 1) * d * N * e));
-            CREATE_TRY(cudaMalloc(&h->r_fk, MS * 2 * d * N * e));
+            CREATE_TRY(dev_malloc(h, &h->r_ft, (MS + 1) * N * e));
+            CREATE_TRY(dev_malloc(h, &h->r_fu, (MS + 1) * d * N * e));
+            CREATE_TRY(dev_malloc(h, &h->r_fk, MS * 2 * d * N * e));
         }
-        CREATE_TRY(cudaMalloc(&h->r_fn, N * sizeof(int32_t)));
-        CREATE_TRY(cudaMalloc(&h->r_rn, N * sizeof(int32_t)));
-        CREATE_TRY(upload_table(&h->d_fwd_saveat, cfg->saveat, (size_t)cfg->K));
+        CREATE_TRY(dev_malloc(h, &h->r_fn, N * sizeof(int32_t)));
+        CREATE_TRY(dev_malloc(h, &h->r_rn, N * sizeof(int32_t)));
+        CREATE_TRY(upload_table(h, &h->d_fwd_saveat, cfg->saveat, (size_t)cfg->K));
     } else {
         const size_t Npad = ((N + block - 1) / block) * block;     // padded checkpoint pitch (whole TMA rows per block)
         h->Npad = (int64_t)Npad;
         const size_t ckpt_rows = ckpt_every > 1 ? ((size_t)S + ckpt_every - 1) / ckpt_every + 1 : (size_t)S + 1;
-        CREATE_TRY(cudaMalloc(&h->d_ckpt, ckpt_rows * d * Npad * e));
+        CREATE_TRY(dev_malloc(h, &h->d_ckpt, ckpt_rows * d * Npad * e));
         h->save_of_step = sos; h->fwd_save_of_step = sos;
-        CREATE_TRY(upload_table(&h->d_save_of_step, sos.data(), sos.size()));
-        CREATE_TRY(upload_table(&h->d_fwd_save_of_step, sos.data(), sos.size()));
-        if (sde) CREATE_TRY(cudaMalloc(&h->d_noise, (size_t)S * m * N * e));
+        CREATE_TRY(upload_table(h, &h->d_save_of_step, sos.data(), sos.size()));
+        CREATE_TRY(upload_table(h, &h->d_fwd_save_of_step, sos.data(), sos.size()));
+        if (sde) CREATE_TRY(dev_malloc(h, &h->d_noise, (size_t)S * m * N * e));
         // BF16_F32ACC = mlp_tc.cuh: member and gradient GEMMs in the time loop on wgmma, fp32 accumulators in registers
-        if (is_mlp_tc(h)) CREATE_TRY(cudaMalloc(&h->d_kst, (size_t)S * 14 * N * sizeof(float)));
+        if (is_mlp_tc(h)) CREATE_TRY(dev_malloc(h, &h->d_kst, (size_t)S * 14 * N * sizeof(float)));
         if (cfg->flags & B200ADJ_FLAG_TRACE) {
-            CREATE_TRY(cudaMalloc(&h->d_trace, (size_t)h->grid * 3 * sizeof(unsigned long long)));
+            CREATE_TRY(dev_malloc(h, &h->d_trace, (size_t)h->grid * 3 * sizeof(unsigned long long)));
             CREATE_TRY(cudaMemset(h->d_trace, 0, (size_t)h->grid * 3 * sizeof(unsigned long long)));
         }
         if (!sde) build_tsit5_tables(cfg->dt, &h->tb);
     }
     {   // block partials of the dG/dp reduction; the T5A / ROS reverse kernels may run with blocks as small as one warp (disp_t5a.inc)
         const size_t blocks = ros ? (N + 31) / 32 : (size_t)h->grid;
-        CREATE_TRY(cudaMalloc(&h->d_partials, (h->qpartials_blocks > blocks ? h->qpartials_blocks : blocks) * P * sizeof(double)));
+        CREATE_TRY(dev_malloc(h, &h->d_partials, (h->qpartials_blocks > blocks ? h->qpartials_blocks : blocks) * P * sizeof(double)));
     }
-    CREATE_TRY(cudaMalloc(&h->d_ticket, sizeof(unsigned int)));
+    CREATE_TRY(dev_malloc(h, &h->d_ticket, sizeof(unsigned int)));
     CREATE_TRY(cudaMemset(h->d_ticket, 0, sizeof(unsigned int)));
     if (!cfg->buffers_on_device) CREATE_TRY(alloc_staging(h));
 #undef CREATE_TRY
@@ -581,6 +602,12 @@ int32_t b200adj_set_reverse_options(void* handle, int32_t sensealg, int32_t cost
     if (sensealg < 0 || sensealg > 4 || (cost_kind != B200ADJ_COST_EXPLICIT && cost_kind != B200ADJ_COST_AFFINE)) { h->err = "bad sensealg/cost_kind"; return B200ADJ_ERR_INVALID; }
     if (int32_t rc = check_support(h, sensealg, h->nev > 0, h->cc_on)) return rc;
     CUDA_TRY(h, cudaSetDevice(c.device));
+    if (K >= 0 && h->d_ck) {
+        // checkpointed save intervals: their bounds (the forward save times) must stay the reverse solve's tstops
+        bool same = K == h->fwd_K && (K == 0 || t);
+        for (int k = 0; same && k < K; k++) same = t[k] == h->fwd_saveat[k];
+        if (!same) { h->err = "B200ADJ_FLAG_CHECKPOINT_SAVES: the reverse pass keeps the forward save times (the bounds of the checkpointed intervals)"; return B200ADJ_ERR_UNSUPPORTED; }
+    }
     if (K >= 0) {
         if (K > 0 && !t) { h->err = "null t"; return B200ADJ_ERR_INVALID; }
         std::vector<int32_t> sos;
@@ -602,14 +629,14 @@ int32_t b200adj_set_reverse_options(void* handle, int32_t sensealg, int32_t cost
             h->save_of_step = sos;
         }
         if (K > c.K) {
-            cudaFree(h->d_saveat); h->d_saveat = nullptr; CUDA_TRY(h, cudaMalloc(&h->d_saveat, (size_t)K * sizeof(double)));
-            cudaFree(h->s_dLdu); h->s_dLdu = nullptr;
+            dev_free(h, h->d_saveat); h->d_saveat = nullptr; CUDA_TRY(h, dev_malloc(h, &h->d_saveat, (size_t)K * sizeof(double)));
+            dev_free(h, h->s_dLdu); h->s_dLdu = nullptr;
         }
         if (K > 0) CUDA_TRY(h, cudaMemcpy(h->d_saveat, t, (size_t)K * sizeof(double), cudaMemcpyHostToDevice));
         h->saveat.assign(t, t + K); c.saveat = h->saveat.data(); c.K = K;
     }
     if (!c.buffers_on_device && cost_kind == B200ADJ_COST_EXPLICIT && c.K > 0 && !h->s_dLdu)
-        CUDA_TRY(h, cudaMalloc(&h->s_dLdu, (size_t)c.K * c.d * (size_t)c.N * esz(c)));
+        CUDA_TRY(h, dev_malloc(h, &h->s_dLdu, (size_t)c.K * c.d * (size_t)c.N * esz(c)));
     c.sensealg = sensealg; c.cost_kind = cost_kind; c.cost_a = cost_a; c.cost_b = cost_b;
     for (int j = 0; j < 4; j++) { h->cost_av[j] = cost_a; h->cost_bv[j] = cost_b; }
     h->has_dgdp = false;
@@ -707,26 +734,26 @@ int32_t b200adj_set_events(void* handle, int32_t E, const double* times, const d
         if (!(times[e] > c.t0 && times[e] < c.t1) || (e > 0 && !(times[e] > times[e - 1]))) { h->err = "events: times must be ascending and strictly inside (t0, t1)"; return B200ADJ_ERR_INVALID; }
     CUDA_TRY(h, cudaSetDevice(c.device));
     CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-    cudaFree(h->d_ev_t); cudaFree(h->d_ev_s); cudaFree(h->d_ev_c); cudaFree(h->d_ev_ps); cudaFree(h->d_ev_pc);
-    cudaFree(h->d_ev_ac); cudaFree(h->d_ev_ak); cudaFree(h->d_ev_af); h->d_ev_ac = h->d_ev_ak = nullptr; h->d_ev_af = nullptr;
+    dev_free(h, h->d_ev_t); dev_free(h, h->d_ev_s); dev_free(h, h->d_ev_c); dev_free(h, h->d_ev_ps); dev_free(h, h->d_ev_pc);
+    dev_free(h, h->d_ev_ac); dev_free(h, h->d_ev_ak); dev_free(h, h->d_ev_af); h->d_ev_ac = h->d_ev_ak = nullptr; h->d_ev_af = nullptr;
     h->d_ev_t = h->d_ev_s = h->d_ev_c = h->d_ev_ps = h->d_ev_pc = nullptr; h->nev = 0; h->have_forward = false;
     if (E > 0) {
-        CUDA_TRY(h, cudaMalloc(&h->d_ev_t, (size_t)E * sizeof(double)));
-        CUDA_TRY(h, cudaMalloc(&h->d_ev_s, (size_t)E * c.d * sizeof(double)));
-        CUDA_TRY(h, cudaMalloc(&h->d_ev_c, (size_t)E * c.d * sizeof(double)));
+        CUDA_TRY(h, dev_malloc(h, &h->d_ev_t, (size_t)E * sizeof(double)));
+        CUDA_TRY(h, dev_malloc(h, &h->d_ev_s, (size_t)E * c.d * sizeof(double)));
+        CUDA_TRY(h, dev_malloc(h, &h->d_ev_c, (size_t)E * c.d * sizeof(double)));
         CUDA_TRY(h, cudaMemcpy(h->d_ev_t, times, (size_t)E * sizeof(double), cudaMemcpyHostToDevice));
         CUDA_TRY(h, cudaMemcpy(h->d_ev_s, scale, (size_t)E * c.d * sizeof(double), cudaMemcpyHostToDevice));
         CUDA_TRY(h, cudaMemcpy(h->d_ev_c, shift, (size_t)E * c.d * sizeof(double), cudaMemcpyHostToDevice));
         if (pscale) {
-            CUDA_TRY(h, cudaMalloc(&h->d_ev_ps, (size_t)E * c.P * sizeof(double)));
-            CUDA_TRY(h, cudaMalloc(&h->d_ev_pc, (size_t)E * c.P * sizeof(double)));
+            CUDA_TRY(h, dev_malloc(h, &h->d_ev_ps, (size_t)E * c.P * sizeof(double)));
+            CUDA_TRY(h, dev_malloc(h, &h->d_ev_pc, (size_t)E * c.P * sizeof(double)));
             CUDA_TRY(h, cudaMemcpy(h->d_ev_ps, pscale, (size_t)E * c.P * sizeof(double), cudaMemcpyHostToDevice));
             CUDA_TRY(h, cudaMemcpy(h->d_ev_pc, pshift, (size_t)E * c.P * sizeof(double), cudaMemcpyHostToDevice));
         }
         h->nev = E;
     }
     if (fixed) {
-        if (!h->d_event_of_step) CUDA_TRY(h, cudaMalloc(&h->d_event_of_step, ((size_t)h->S + 1) * sizeof(int32_t)));
+        if (!h->d_event_of_step) CUDA_TRY(h, dev_malloc(h, &h->d_event_of_step, ((size_t)h->S + 1) * sizeof(int32_t)));
         CUDA_TRY(h, cudaMemcpy(h->d_event_of_step, eos.data(), eos.size() * sizeof(int32_t), cudaMemcpyHostToDevice));
     }
     return B200ADJ_OK;
@@ -739,7 +766,7 @@ int32_t b200adj_set_event_param_shift(void* handle, const int32_t* comp, const i
     if (h->nev <= 0) { h->err = "event parameter shift: call b200adj_set_events first"; return B200ADJ_ERR_STATE; }
     CUDA_TRY(h, cudaSetDevice(c.device));
     CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-    cudaFree(h->d_ev_ac); cudaFree(h->d_ev_ak); cudaFree(h->d_ev_af); h->d_ev_ac = h->d_ev_ak = nullptr; h->d_ev_af = nullptr;
+    dev_free(h, h->d_ev_ac); dev_free(h, h->d_ev_ak); dev_free(h, h->d_ev_af); h->d_ev_ac = h->d_ev_ak = nullptr; h->d_ev_af = nullptr;
     h->have_forward = false;
     if (!comp) return B200ADJ_OK;                                      // removes the shifts
     if (!param || !coef) { h->err = "event parameter shift: null argument"; return B200ADJ_ERR_INVALID; }
@@ -750,9 +777,9 @@ int32_t b200adj_set_event_param_shift(void* handle, const int32_t* comp, const i
         if (comp[e] >= c.d || (comp[e] >= 0 && (param[e] < 0 || param[e] >= c.P || !std::isfinite(coef[e])))) {
             h->err = "event parameter shift: bad component / parameter index"; return B200ADJ_ERR_INVALID; }
     const size_t E = (size_t)h->nev;
-    CUDA_TRY(h, cudaMalloc(&h->d_ev_ac, E * sizeof(int32_t)));
-    CUDA_TRY(h, cudaMalloc(&h->d_ev_ak, E * sizeof(int32_t)));
-    CUDA_TRY(h, cudaMalloc(&h->d_ev_af, E * sizeof(double)));
+    CUDA_TRY(h, dev_malloc(h, &h->d_ev_ac, E * sizeof(int32_t)));
+    CUDA_TRY(h, dev_malloc(h, &h->d_ev_ak, E * sizeof(int32_t)));
+    CUDA_TRY(h, dev_malloc(h, &h->d_ev_af, E * sizeof(double)));
     CUDA_TRY(h, cudaMemcpy(h->d_ev_ac, comp, E * sizeof(int32_t), cudaMemcpyHostToDevice));
     CUDA_TRY(h, cudaMemcpy(h->d_ev_ak, param, E * sizeof(int32_t), cudaMemcpyHostToDevice));
     CUDA_TRY(h, cudaMemcpy(h->d_ev_af, coef, E * sizeof(double), cudaMemcpyHostToDevice));
@@ -898,6 +925,12 @@ int32_t b200adj_synchronize(void* handle) {
 }
 
 int64_t b200adj_launch_count(void* handle) { return handle ? ((Handle*)handle)->launches : -1; }
+
+int32_t b200adj_device_bytes(void* handle, int64_t* bytes) {
+    if (!handle || !bytes) return B200ADJ_ERR_INVALID;
+    *bytes = ((Handle*)handle)->dev_bytes;
+    return B200ADJ_OK;
+}
 
 int32_t b200adj_get_step_counts(void* handle, int32_t* fwd_steps, int32_t* rev_steps) {
     if (!handle) return B200ADJ_ERR_INVALID;

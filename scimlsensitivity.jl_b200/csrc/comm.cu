@@ -79,12 +79,12 @@ static void p2p_point(P2PComm* pc, int r, void* base) {
 }
 static void p2p_release(Handle* h) {
     for (int r = 0; r < P2P_MAXRANKS; r++) if (h->p2p_ipc_open[r]) { cudaIpcCloseMemHandle(h->p2p_ipc_open[r]); h->p2p_ipc_open[r] = nullptr; }
-    if (h->p2p_mailbox) { cudaFree(h->p2p_mailbox); h->p2p_mailbox = nullptr; }
+    dev_free(h, h->p2p_mailbox);
     memset(&h->p2p, 0, sizeof(h->p2p)); h->p2p_epoch = 0;
 }
 static bool p2p_alloc(Handle* h) {
     if (cudaSetDevice(h->cfg.device) != cudaSuccess) return false;
-    if (cudaMalloc(&h->p2p_mailbox, P2P_MAILBOX_BYTES) != cudaSuccess) { cudaGetLastError(); h->p2p_mailbox = nullptr; return false; }
+    if (dev_malloc(h, &h->p2p_mailbox, P2P_MAILBOX_BYTES) != cudaSuccess) { cudaGetLastError(); h->p2p_mailbox = nullptr; return false; }
     return cudaMemset(h->p2p_mailbox, 0, P2P_MAILBOX_BYTES) == cudaSuccess && cudaDeviceSynchronize() == cudaSuccess;
 }
 // one process per GPU: exchange CUDA IPC handles of the mailboxes through the communicator itself (one ncclAllGather)

@@ -11,6 +11,7 @@
 
 #include <string>
 #include <type_traits>
+#include <unordered_map>
 #include <vector>
 
 #include "../../include/b200adj.h"
@@ -52,7 +53,11 @@ struct Handle {
     unsigned long long* d_trace = nullptr;   // [grid][3] block trace (B200ADJ_FLAG_TRACE)
     unsigned int* d_ticket = nullptr;
     int32_t* d_save_of_step = nullptr;
-    int maxs = 0;                     // T5A / ROS: per-member step capacity of the dense forward / reverse solutions
+    int maxs = 0;                     // T5A / ROS: per-member step capacity of the dense forward / reverse solutions (T5A with
+                                      // B200ADJ_FLAG_CHECKPOINT_SAVES: of ONE save interval)
+    // T5A, B200ADJ_FLAG_CHECKPOINT_SAVES: the checkpoint of every save interval, [N][ck_nseg][2 d + 4] (tsit5_adaptive.cuh,
+    // t5a_ckpt); the intervals are bounded by t0, the save times inside (t0, t1) -- saveat[ck_k0 ..] -- and t1
+    double* d_ck = nullptr; int ck_nseg = 0, ck_k0 = 0;
     double adj_abstol = 0, adj_reltol = 0;   // <= 0: use the forward tolerances
     // named cost family, per component (b200adj_set_cost_family; the scalar entry points broadcast):
     //   discrete (COST_AFFINE)  dgdu = cost_av .* u + cost_bv,  dgdp = dgdp_c .* p + dgdp_e   at every save time
@@ -100,7 +105,23 @@ struct Handle {
     void* p2p_ipc_open[P2P_MAXRANKS] = {nullptr};   // cudaIpcOpenMemHandle mappings to close
     unsigned long long p2p_epoch = 0;
     std::string err;
+    // the device memory the handle owns (b200adj_device_bytes): every allocation goes through dev_malloc / dev_free
+    int64_t dev_bytes = 0;
+    std::unordered_map<const void*, size_t> dev_sizes;
 };
+
+template <class T> cudaError_t dev_malloc(Handle* h, T** p, size_t bytes) {
+    const cudaError_t e = cudaMalloc((void**)p, bytes);
+    if (e == cudaSuccess) { h->dev_sizes[*p] = bytes; h->dev_bytes += (int64_t)bytes; }
+    return e;
+}
+template <class T> void dev_free(Handle* h, T*& p) {
+    if (!p) return;
+    const auto it = h->dev_sizes.find(p);
+    if (it != h->dev_sizes.end()) { h->dev_bytes -= (int64_t)it->second; h->dev_sizes.erase(it); }
+    cudaFree((void*)p);
+    p = nullptr;
+}
 
 #define CUDA_TRY(h, expr)                                                                      \
     do {                                                                                       \

@@ -60,6 +60,12 @@ struct T5aArgs {
     // fe_nc > 0 selects them; fe_dir[c] is the direction of condition c (-1 down, +1 up, 0 both).
     int32_t fe_nc, fe_dir[8];
     int32_t* cc_ev;
+    // checkpointed save intervals (CK, B200ADJ_FLAG_CHECKPOINT_SAVES): segment s runs from bound s to bound s + 1, the bounds
+    // being t0, saveat[ck_k0 .. ck_k0 + ck_nseg - 2] (the save times inside (t0, t1)) and t1.  The forward kernel writes no
+    // dense records, only ck[N][ck_nseg][2 D + 4] (t5a_ckpt); the reverse kernel re-solves one segment at a time into
+    // frecT / ftT, whose rows then hold maxs + 1 records of ONE segment.  ck_abstol / ck_reltol: the forward tolerances
+    // (abstol / reltol may be the adjoint's in the reverse pass).
+    double* ck; int32_t ck_nseg, ck_k0; double ck_abstol, ck_reltol;
 };
 
 // a family struct carries conditions and an affect (family_plugin.inc specialises this for B200ADJ_FAMILY_HAS_EVENTS)
@@ -183,7 +189,8 @@ __device__ __forceinline__ void t5_step(const T5aArgs& a, const RHS& rhs, double
     }
 }
 template <int L>
-__device__ __forceinline__ double t5_error(const T5aArgs& a, double h, const double* z, const double* zn, const double (*k)[L]) {
+__device__ __forceinline__ double t5_error_tol(const T5aArgs& a, double atol, double rtol, double h, const double* z, const double* zn,
+                                               const double (*k)[L]) {
     double e2 = 0;
 #pragma unroll
     for (int c = 0; c < L; c++) {
@@ -191,11 +198,81 @@ __device__ __forceinline__ double t5_error(const T5aArgs& a, double h, const dou
 #pragma unroll
         for (int j = 0; j < 7; j++) e += a.BT[j] * k[j][c];
         e *= h;
-        const double sc = a.abstol + a.reltol * fmax(fabs(z[c]), fabs(zn[c]));
+        const double sc = atol + rtol * fmax(fabs(z[c]), fabs(zn[c]));
         e2 += (e / sc) * (e / sc);
     }
     return sqrt(e2 / L);
 }
+template <int L>
+__device__ __forceinline__ double t5_error(const T5aArgs& a, double h, const double* z, const double* zn, const double (*k)[L]) {
+    return t5_error_tol<L>(a, a.abstol, a.reltol, h, z, zn, k);
+}
+
+// One attempt of the forward step from (t, u) with k[0] = f(u) given: the step is clipped at tend (last), then the embedded
+// error estimate and the PI controller decide.  T5_ACCEPT: un and k[1..6] hold the step, EEst and q update the controller
+// (qold = max(EEst, 1e-4), h = h / q); T5_REJECT: h has shrunk, try again; T5_DTMIN: a trial step overflowed and h fell
+// below dtmin.  The forward kernel and the reverse kernel's replay of a save interval (CK) both step through this function,
+// so the replay takes the forward steps bit for bit.
+enum { T5_REJECT = 0, T5_ACCEPT = 1, T5_DTMIN = 2 };
+template <int D, class RHS>
+__device__ __forceinline__ int t5a_attempt(const T5aArgs& a, const RHS& rhs, double atol, double rtol, bool fixed, double t, double tend,
+                                           double& h, double qold, const double* u, double (*k)[D], double* un, bool& last,
+                                           double& EEst, double& q) {
+    last = false;
+    if (t + h >= tend || fabs(t + h - tend) < 100 * 2.22e-16 * fabs(tend)) { h = tend - t; last = true; }
+    t5_step<D>(a, rhs, t, h, u, k, un);
+    EEst = fixed ? 0.0 : t5_error_tol<D>(a, atol, rtol, h, u, un, k);
+    if (!isfinite(EEst)) {                    // a trial step that overflowed: shrink (OrdinaryDiffEq does), give up below dtmin
+        h *= 0.25;
+        return (fabs(h) > 1e-14 * fmax(fabs(t), fabs(a.t1 - a.t0))) ? T5_REJECT : T5_DTMIN;
+    }
+    const double q11 = pow(fmax(EEst, 1e-300), 7.0 / 50.0);
+    q = q11 / pow(qold, 2.0 / 25.0);
+    q = fmax(1.0 / 10.0, fmin(5.0, q / 0.9));
+    if (EEst <= 1.0) return T5_ACCEPT;
+    h = h / fmin(5.0, q11 / 0.9);
+    return T5_REJECT;
+}
+
+// The record of an accepted step [t, tn] (start state, k1..k7, knots), staged in shared memory st, then ONE bulk store to rec
+template <int D>
+__device__ __forceinline__ void t5a_put_record(const T5aArgs& a, double* st, double* rec, const double* u, const double (*k)[D], double t, double tn) {
+    constexpr int REC = t5_rec<D>();
+    tma_store_wait_read();                                 // the previous record has left the staging buffer
+#pragma unroll
+    for (int j = 0; j < D; j++) st[j] = u[j];
+    // the stages enter the record as the coefficients of the interpolant in powers of theta,
+    //   y(theta) = u_n + h theta (c0 + theta (c1 + theta (c2 + theta c3))),  c_m = sum_s R[s][m] k_s
+    // (b_s(theta) = sum_m R[s][m] theta^(m+1)): computed once here, every lookup of the reverse solve and of the
+    // quadrature is then 4 FMAs per component instead of the seven weights + a 7-term combination
+#pragma unroll
+    for (int j = 0; j < D; j++) {
+#pragma unroll
+        for (int m = 0; m < 4; m++) {
+            double c = 0.0;
+#pragma unroll
+            for (int s = 0; s < 7; s++) c += a.R[s][m] * k[s][j];
+            st[D + m * D + j] = c;
+        }
+#pragma unroll
+        for (int m = 4; m < 7; m++) st[D + m * D + j] = 0.0;
+    }
+    const double hrec = tn - t;
+    st[8 * D] = t; st[8 * D + 1] = hrec; st[8 * D + 2] = 1.0 / hrec; st[8 * D + 3] = tn;
+    fence_proxy_async_smem();
+    tma_store_1d(rec, st, (uint32_t)(REC * sizeof(double)));
+    tma_store_commit();
+}
+
+// CK: the bounds of the save intervals and member i's checkpoint of interval s, (t_n, h of the first attempt, qold, n, u_n[D],
+// k1 = f(u_n)[D]) of the accepted forward step n whose interval [t_n, t_n+1] holds the lower bound (t_n < bound <= t_n+1;
+// step 0 for the interval at t0)
+template <int D> __host__ __device__ constexpr int t5_ckw() { return 2 * D + 4; }
+__device__ __forceinline__ double t5a_bound(const T5aArgs& a, int s) {
+    return s <= 0 ? a.t0 : (s >= a.ck_nseg ? a.t1 : a.saveat[a.ck_k0 + s - 1]);
+}
+template <int D>
+__device__ __forceinline__ double* t5a_ckpt(const T5aArgs& a, int64_t i, int s) { return a.ck + (i * a.ck_nseg + s) * t5_ckw<D>(); }
 
 // effective affine affect of the state-dependent event for a member with parameters p (constant along the solve)
 template <int D, int P>
@@ -392,8 +469,20 @@ __device__ __forceinline__ uint32_t t5_fire_reached(const Event& event, const do
     return word;
 }
 
-// CC: continuous callback, its conditions and affect those of the policy T5Event<Fam, FE>: the family's (FE) or the named one
-template <class Fam, bool SHARED_P, bool CC = false, bool FE = false>
+// CK: write member i's checkpoint of save interval s
+template <int D>
+__device__ __forceinline__ void t5a_put_ckpt(const T5aArgs& a, int64_t i, int s, double t, double h, double qold, int n, const double* u,
+                                             const double* k0) {
+    double* c = t5a_ckpt<D>(a, i, s);
+    c[0] = t; c[1] = h; c[2] = qold; c[3] = (double)n;
+#pragma unroll
+    for (int j = 0; j < D; j++) { c[4 + j] = u[j]; c[4 + D + j] = k0[j]; }
+}
+
+// CC: continuous callback, its conditions and affect those of the policy T5Event<Fam, FE>: the family's (FE) or the named one.
+// CK: checkpointed save intervals -- no dense records, the checkpoint of every save interval instead (t5a_ckpt), and the step
+// capacity maxs counts the steps of one interval's replay (t5a_replay)
+template <class Fam, bool SHARED_P, bool CC = false, bool FE = false, bool CK = false>
 __global__ void __launch_bounds__(256) t5a_forward_kernel(const __grid_constant__ T5aArgs a) {
     constexpr int D = Fam::D, P = Fam::P;
     using Event = T5Event<Fam, FE>;
@@ -412,12 +501,17 @@ __global__ void __launch_bounds__(256) t5a_forward_kernel(const __grid_constant_
     double u[D], un[D], k[7][D];
 #pragma unroll
     for (int j = 0; j < D; j++) u[j] = a.u0[(int64_t)j * N + i];
-    knots[0] = a.t0;
+    if constexpr (!CK) knots[0] = a.t0;
     auto rhs = [&](double, const double* x, double* dx) { Fam::f(x, p, dx); };
     Fam::f(u, p, k[0]);
     double t = a.t0, h = a.dt0 > 0 ? a.dt0 : 1e-3 * (a.t1 - a.t0), qold = 1e-4;
     int n = 0, ksave = 0, stat = 0;
     long iters = 0;
+    // CK: next checkpoint to write; the lowest save interval whose replay still runs through the coming step (its upper bound
+    // not passed yet) and the step its checkpoint starts at; the first-attempt step size of the coming step
+    int cks = 1, slo = 0, nlo = 0;
+    double h1 = h;
+    if constexpr (CK) t5a_put_ckpt<D>(a, i, 0, t, h, qold, 0, u, k[0]);
     while (a.saved && ksave < a.K && a.saveat[ksave] <= a.t0) {
 #pragma unroll
         for (int j = 0; j < D; j++) a.saved[((int64_t)ksave * D + j) * N + i] = u[j];
@@ -428,21 +522,16 @@ __global__ void __launch_bounds__(256) t5a_forward_kernel(const __grid_constant_
     int nfound = 0;
     uint32_t cc_skip = 0, cc_word = 0;            // CC: conditions that fired at the event the step starts on; the event word
     while (t < a.t1) {
-        if (++iters > 10000000L || n >= a.maxs) { stat = 2; break; }
-        bool last = false;
-        const double tend = (!CC && ev < a.nev) ? a.ev_t[ev] : a.t1;
-        if (t + h >= tend || fabs(t + h - tend) < 100 * 2.22e-16 * fabs(tend)) { h = tend - t; last = true; }
-        t5_step<D>(a, rhs, t, h, u, k, un);
-        const double EEst = fixed ? 0.0 : t5_error<D>(a, h, u, un, k);
-        if (!isfinite(EEst)) {                    // a trial step that overflowed: shrink (OrdinaryDiffEq does), give up below dtmin
-            h *= 0.25;
-            if (!(fabs(h) > 1e-14 * fmax(fabs(t), fabs(a.t1 - a.t0)))) { stat = 1; break; }
-            continue;
+        if constexpr (CK) {
+            while (slo + 1 < a.ck_nseg && t5a_bound(a, slo + 1) < t) { slo++; nlo = (int)t5a_ckpt<D>(a, i, slo)[3]; }
         }
-        const double q11 = pow(fmax(EEst, 1e-300), 7.0 / 50.0);
-        double q = q11 / pow(qold, 2.0 / 25.0);
-        q = fmax(1.0 / 10.0, fmin(5.0, q / 0.9));
-        if (EEst <= 1.0) {
+        if (++iters > 10000000L || (CK ? n - nlo >= a.maxs : n >= a.maxs)) { stat = 2; break; }
+        bool last;
+        double EEst, q;
+        const double tend = (!CC && ev < a.nev) ? a.ev_t[ev] : a.t1;
+        const int r = t5a_attempt<D>(a, rhs, a.abstol, a.reltol, fixed, t, tend, h, qold, u, k, un, last, EEst, q);
+        if (r == T5_DTMIN) { stat = 1; break; }
+        if (r == T5_ACCEPT) {
             double tn = last ? tend : t + h;
             bool at_event = !CC && last && ev < a.nev;
             if constexpr (CC) {
@@ -469,6 +558,9 @@ __global__ void __launch_bounds__(256) t5a_forward_kernel(const __grid_constant_
                     nfound++;
                 }
             }
+            if constexpr (CK) {           // the save intervals whose lower bound this step holds start with it
+                while (cks < a.ck_nseg && t5a_bound(a, cks) <= tn) { t5a_put_ckpt<D>(a, i, cks, t, h1, qold, n, u, k[0]); cks++; }
+            }
             // a save time that coincides with an event records the post-event state (saved after the affect, below)
             while (a.saved && ksave < a.K && (a.saveat[ksave] < tn || (a.saveat[ksave] == tn && !at_event))) {
                 const double hh = tn - t, th = (hh == 0.0) ? 1.0 : (a.saveat[ksave] - t) / hh;
@@ -483,32 +575,8 @@ __global__ void __launch_bounds__(256) t5a_forward_kernel(const __grid_constant_
                 }
                 ksave++;
             }
-            {   // the step's record (start state, k1..k7, knots): staged in shared memory, then ONE bulk store to this member's row
-                tma_store_wait_read();                                 // the previous record has left the staging buffer
-#pragma unroll
-                for (int j = 0; j < D; j++) st[j] = u[j];
-                // the stages enter the record as the coefficients of the interpolant in powers of theta,
-                //   y(theta) = u_n + h theta (c0 + theta (c1 + theta (c2 + theta c3))),  c_m = sum_s R[s][m] k_s
-                // (b_s(theta) = sum_m R[s][m] theta^(m+1)): computed once here, every lookup of the reverse solve and of the
-                // quadrature is then 4 FMAs per component instead of the seven weights + a 7-term combination
-#pragma unroll
-                for (int j = 0; j < D; j++) {
-#pragma unroll
-                    for (int m = 0; m < 4; m++) {
-                        double c = 0.0;
-#pragma unroll
-                        for (int s = 0; s < 7; s++) c += a.R[s][m] * k[s][j];
-                        st[D + m * D + j] = c;
-                    }
-#pragma unroll
-                    for (int m = 4; m < 7; m++) st[D + m * D + j] = 0.0;
-                }
-                const double hrec = tn - t;
-                st[8 * D] = t; st[8 * D + 1] = hrec; st[8 * D + 2] = 1.0 / hrec; st[8 * D + 3] = tn;
-                fence_proxy_async_smem();
-                tma_store_1d(recs + (int64_t)n * REC, st, (uint32_t)(REC * sizeof(double)));
-                tma_store_commit();
-            }
+            // the step's record: ONE bulk store to this member's row
+            if constexpr (!CK) t5a_put_record<D>(a, st, recs + (int64_t)n * REC, u, k, t, tn);
             if (at_event) {
                 // affect!: the next step starts from the post-event state; k7 = f(u^-) stays with the step just stored
                 if constexpr (CC) {
@@ -549,16 +617,16 @@ __global__ void __launch_bounds__(256) t5a_forward_kernel(const __grid_constant_
             }
 #pragma unroll
             for (int j = 0; j < D; j++) { u[j] = un[j]; k[0][j] = k[6][j]; }
-            t = tn; knots[n + 1] = t;
+            t = tn;
+            if constexpr (!CK) knots[n + 1] = t;
             n++;
             qold = fmax(EEst, 1e-4);
             h = fixed ? a.dt0 : h / q;            // constant step: back to dt after a step clipped at an event (dtcache)
-        } else {
-            h = h / fmin(5.0, q11 / 0.9);
+            h1 = h;
         }
     }
     a.fn[i] = n;
-    {   // the terminal record: final state and time
+    if constexpr (!CK) {   // the terminal record: final state and time
         tma_store_wait_read();
 #pragma unroll
         for (int j = 0; j < D; j++) st[j] = u[j];
@@ -578,6 +646,47 @@ __global__ void __launch_bounds__(256) t5a_forward_kernel(const __grid_constant_
     if (a.status) a.status[i] = stat;
 }
 
+// CK: re-solve save interval s of member i from its checkpoint with the forward kernel's step (t5a_attempt, the forward
+// tolerances) into the member's one-interval dense solution: records staged in st and bulk-stored as the forward kernel does,
+// knots.  The replay runs until a step has passed the interval's upper bound (to t1 in the last interval), so that a lookup
+// anywhere in [lower bound, upper bound], right- or left-continuous, selects the forward step the full dense solution would:
+// the step that straddles a save time belongs to both intervals.  Returns the number of records, -1 when the interval needs
+// more than maxs steps.  On return every record is in global memory (the lookups read them with bulk copies).
+template <class Fam>
+__device__ __forceinline__ int t5a_replay(const T5aArgs& a, int64_t i, int s, const double* p, double* st, double* recs, double* knots) {
+    constexpr int D = Fam::D, REC = t5_rec<D>();
+    const double* c = t5a_ckpt<D>(a, i, s);
+    double u[D], un[D], k[7][D];
+    double t = c[0], h = c[1], qold = c[2];
+#pragma unroll
+    for (int j = 0; j < D; j++) { u[j] = c[4 + j]; k[0][j] = c[4 + D + j]; }
+    const double tup = t5a_bound(a, s + 1);
+    auto rhs = [&](double, const double* x, double* dx) { Fam::f(x, p, dx); };
+    const bool fixed = (a.flags & KF_FIXED_DT) != 0;
+    int m = 0;
+    knots[0] = t;
+    while (t < a.t1 && t <= tup) {
+        if (m >= a.maxs) { m = -1; break; }
+        bool last;
+        double EEst, q;
+        const int r = t5a_attempt<D>(a, rhs, a.ck_abstol, a.ck_reltol, fixed, t, a.t1, h, qold, u, k, un, last, EEst, q);
+        if (r == T5_DTMIN) { m = -1; break; }
+        if (r != T5_ACCEPT) continue;
+        const double tn = last ? a.t1 : t + h;
+        t5a_put_record<D>(a, st, recs + (int64_t)m * REC, u, k, t, tn);
+#pragma unroll
+        for (int j = 0; j < D; j++) { u[j] = un[j]; k[0][j] = k[6][j]; }
+        t = tn;
+        knots[m + 1] = t;
+        m++;
+        qold = fmax(EEst, 1e-4);
+        h = fixed ? a.dt0 : h / q;
+    }
+    tma_store_wait_all();
+    asm volatile("fence.proxy.async.global;" ::: "memory");      // the bulk stores, then the bulk loads of the lookups
+    return m;
+}
+
 // reverse adjoint solve.  SA_INTERP: z = [lambda; mu] (L = D + P); SA_GAUSS / SA_QUAD: z = lambda (L = D);
 // SA_BACKSOLVE: z = [lambda; mu; y] (L = 2D + P), y integrated backwards and reset from the forward solution at the
 // checkpoints (every forward knot = sol.t, the direct-interface default, or the save times), which are tstops of the reverse
@@ -586,7 +695,9 @@ __global__ void __launch_bounds__(256) t5a_forward_kernel(const __grid_constant_
 // (A register cap -- __maxnreg__(144): 14 warps per SM, the 65 536-member C1 shard in ONE wave instead of two -- was measured
 // twice and rejected: 8.9 ms against 7.25 ms uncapped.  Block sizes 32 / 64 / 128 (8 to 11 resident warps per SM) all give
 // 7.25 ms: the time is two rounds of a latency-bound per-warp chain, see DESIGN.md 4.4.)
-template <class Fam, int SA, bool SHARED_P, int COST, bool CC = false, bool FE = false>
+// CK: checkpointed save intervals -- entering each save interval (at t1, and after the jump at each save time) the kernel
+// re-solves it from its checkpoint into this member's rows of frecT / ftT (t5a_replay) and points the dense lookups at it
+template <class Fam, int SA, bool SHARED_P, int COST, bool CC = false, bool FE = false, bool CK = false>
 __global__ void __launch_bounds__(256) t5a_reverse_kernel(const __grid_constant__ T5aArgs a) {
     constexpr int D = Fam::D, P = Fam::P, L = (SA == SA_INTERP) ? D + P : (SA == SA_BACKSOLVE ? 2 * D + P : D);
     constexpr int YO = (SA == SA_BACKSOLVE) ? D + P : 0;          // offset of y inside z (Backsolve)
@@ -609,7 +720,7 @@ __global__ void __launch_bounds__(256) t5a_reverse_kernel(const __grid_constant_
     uint64_t* my_bar = reinterpret_cast<uint64_t*>(s_t5_dense + (size_t)2 * bufstride) + threadIdx.x;
     mbar_init(my_bar, 1);
     mbar_fence_init();
-    T5Dense<D> sol{a, a.frecT + (int64_t)i * (a.maxs + 1) * REC, a.ftT + (int64_t)i * (a.maxs + 1), a.fn[i],
+    T5Dense<D> sol{a, a.frecT + (int64_t)i * (a.maxs + 1) * REC, a.ftT + (int64_t)i * (a.maxs + 1), CK ? 0 : a.fn[i],
                    s_t5_dense + (size_t)threadIdx.x * t5_pitch<D>(), bufstride, my_bar};
     sol.cur = sol.n - 1;
     double z[L], zn[L], k[7][L];
@@ -645,7 +756,8 @@ __global__ void __launch_bounds__(256) t5a_reverse_kernel(const __grid_constant_
     int cur = a.K - 1, nrev = 0, ck = sol.n, evc = (CC ? a.cc_n[i] : a.nev) - 1;
     // a member whose forward solve stopped before t1 (status 1 / 2 / 3) has records only up to the break: NaN, as for a
     // reverse solve that overflows, not the gradient of a trajectory that was never solved
-    bool fsal_ok = false, overflow = a.status[i] != 0;
+    // (CK: a thread past the last member would replay member N - 1 into the rows that member's own thread reads)
+    bool fsal_ok = false, overflow = a.status[i] != 0 || (CK && !active);
     const bool ckpt_on = !(a.flags & KF_NO_CHECKPOINTING), every = (a.flags & KF_CKPT_EVERY_STEP);
     if (SA == SA_BACKSOLVE) {
 #pragma unroll
@@ -765,6 +877,16 @@ __global__ void __launch_bounds__(256) t5a_reverse_kernel(const __grid_constant_
             cur--; fsal_ok = false;
         }
     };
+    // CK: the save interval the solve is in; entering interval s re-solves it and resets the lookups onto its records (no
+    // bulk copy into the record buffers may be in flight while the replay stages its records in one of them)
+    int seg = a.ck_nseg - 1;
+    auto enter = [&](int s) {
+        if (sol.aiv >= 0) sol.arrived();
+        const int m = t5a_replay<Fam>(a, i, s, p, sol.sc, a.frecT + i * (a.maxs + 1) * REC, a.ftT + i * (a.maxs + 1));
+        if (m < 0) overflow = true;
+        sol.n = m > 0 ? m : 0; sol.cur = sol.n - 1; sol.cb = 0; sol.civ = -1; sol.aiv = -1;
+    };
+    if constexpr (CK) { if (!overflow) enter(seg); }
     ckpt_if_at(t);
     jump_if_at(t);
     double h = a.dt0 > 0 ? -a.dt0 : -1e-4 * (T - t0), qold = 1e-4;
@@ -853,6 +975,9 @@ __global__ void __launch_bounds__(256) t5a_reverse_kernel(const __grid_constant_
         ckpt_if_at(t);
         jump_if_at(t);
         event_if_at(t);
+        if constexpr (CK) {
+            if (seg > 0 && t <= t5a_bound(a, seg)) { seg--; enter(seg); }
+        }
     }
     // the record of the interval below the last lookup may still be on its way (Backsolve's last checkpoint above t0, a
     // member that stops early): no bulk copy may outlive the CTA whose shared memory it writes

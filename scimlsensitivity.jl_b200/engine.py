@@ -20,7 +20,7 @@ class DeviceEnsemble:
                  on_device=False, device=0, no_start=False, checkpointing=True, ckpt_every_step=False,
                  stored_noise=False, seed=0, traj_offset=0, block_threads=0, abstol=1e-6, reltol=1e-3,
                  quad_abstol=1e-6, quad_reltol=1e-3, dtype="f64", trace=False, max_steps=0, pin_outputs=False,
-                 checkpoint_every=1, no_rotate=False, dense_forward=False, nccl_allreduce=False):
+                 checkpoint_every=1, no_rotate=False, dense_forward=False, nccl_allreduce=False, checkpoint_saves=False):
         d, P, m = FAMILIES[family]
         cfg = _lib.Cfg()
         cfg.rhs_family, cfg.sensealg, cfg.stepper, cfg.dtype = _lib.FAM[family], _lib.SA[sensealg], _lib.ST[stepper], _lib.DTYPE[dtype]
@@ -56,6 +56,10 @@ class DeviceEnsemble:
             flags |= _lib.FLAG_DENSE_FORWARD
         if nccl_allreduce:
             flags |= _lib.FLAG_NCCL_ALLREDUCE
+        if checkpoint_saves:
+            # adaptive Tsit5: keep one checkpoint per save interval, re-solve each interval in the reverse pass (max_steps
+            # then sizes ONE interval); the gradients are those of the full dense solution, bit for bit
+            flags |= _lib.FLAG_CHECKPOINT_SAVES
         cfg.flags, cfg.block_threads = flags, int(block_threads)
         self.family, self.d, self.P, self.m, self.N, self.K = family, d, P, m, int(N), len(saveat)
         self.shared_p, self.on_device, self.device = bool(shared_p), bool(on_device), int(device)
@@ -231,6 +235,10 @@ class DeviceEnsemble:
         out = self._empty(self.S, self.m, self.N, role="noise")
         self.handle.get_noise(out)
         return out
+
+    def device_bytes(self):
+        """Device memory the handle owns now, in bytes."""
+        return self.handle.device_bytes()
 
     def close(self):
         self.handle.close()

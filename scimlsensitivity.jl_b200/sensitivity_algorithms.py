@@ -119,6 +119,9 @@ class B200Adjoint(AbstractAdjointSensitivityAlgorithm):
     stored_noise: bool = False
     checkpoint_every: int = 1     # fixed-step Tsit5 with inner.checkpointing: keep the forward state every C steps and re-solve
                                   # each segment in the reverse pass (the reference's `checkpoints` grid, src/interpolating_adjoint.jl:54-112)
+    checkpoint_saves: bool = False  # adaptive Tsit5: keep one checkpoint per save interval and re-solve each interval in the reverse
+                                    # pass (CheckpointSolution, src/interpolating_adjoint.jl:40-112); bit-identical gradients, memory
+                                    # per member ~ one interval's steps (`maxiters` then bounds ONE interval)
 
     def __post_init__(self):
         if self.inner is None:
